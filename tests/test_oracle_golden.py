@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 import common
+import model64
 from oracle import oracle
 
 GOLDEN = sorted(p for p in glob.glob(os.path.join(os.path.dirname(__file__), "golden", "*.npz"))
@@ -35,6 +36,16 @@ def test_oracle_reproduces_reference_kernel_outputs(path):
         # fp16 mode rounds rgba to half and accumulates with order-dependent half adds
         np.testing.assert_allclose(fwd["rgba"].astype(np.float32), z["out_rgba"].astype(np.float32),
                                    rtol=2e-3, atol=1e-3)
+        # its gradients are half atomics like the reference's: each entry within the float64 model's
+        # half-atomic bound, on the oracle's own saved outputs
+        bwd = oracle.trace_backward(*scene, z["rays"], z["start"], fwd["rgba"], z["grad_rgba"], q,
+                                    fwd.get("depth_indices"), z.get("grad_depth"), None, *settings)
+        m = model64.trace(*scene, z["rays"], z["start"], q, *settings, rgba=fwd["rgba"], grad_rgba=z["grad_rgba"],
+                          grad_depth=z.get("grad_depth"), depth_indices=fwd.get("depth_indices"))
+        skip = model64.rows_reachable(m, z["offsets"], z["adjacency"], z["points"], z["attributes"], z["rays"],
+                                      z["start"], q, *settings)
+        model64.compare({k: np.asarray(bwd[k]) for k in ("points_grad", "attr_grad")}, m, half_atomics=True,
+                        skip_rows=skip, per_ray=False)
         return
     ref = {k[4:]: v for k, v in z.items() if k.startswith("out_")}
     common.assert_forward_close_cpu(fwd, ref, z["attributes"])
