@@ -36,8 +36,10 @@
  *     dtype), point_error[N] (attr dtype, caller zero-initialises).
  *     Unlike the reference, points_grad / attribute_grad are fully
  *     OVERWRITTEN by rfb_trace_backward (no caller zero-fill needed; a
- *     zero-filled buffer gives the same result).  ray_grad is accepted and
- *     never written, exactly like the reference kernel (pipeline.cu:132-343).
+ *     zero-filled buffer gives the same result).  ray_grad[R][6] f32 =
+ *     dL/d(origin, direction as passed in) is opt-in (RFB_FLAG_RAY_GRAD):
+ *     with the flag it is fully overwritten; without it, it is never
+ *     written, like the reference kernel (pipeline.cu:132-343).
  *   - the pipeline object owns only its own scratch (cached, re-laid-out
  *     mirrors of the scene and the fp32 gradient accumulator); it never frees
  *     or retains caller memory beyond a call.
@@ -118,6 +120,11 @@ typedef struct rfb_launch_opts {
  * unchanged since that forward (the library compares the pointers, not the data).  If the tape's
  * memory cannot be allocated the forward simply does not record and the backward re-walks. */
 #define RFB_FLAG_USE_TAPE 4u
+/* trace_backward: also compute ray_grad[r] = dL/d(origin, direction as passed in, before renormalisation),
+ * with the walk's cell sequence held fixed (DESIGN.md §2).  ray_grad is fully overwritten and MUST NOT be NULL;
+ * RFB_FLAG_SCRUB_NONFINITE zeroes its non-finite entries too.  Every other output is the same with or without
+ * it.  (rfb_trace_backward_accumulate_rays takes ray_grad directly instead of this flag.) */
+#define RFB_FLAG_RAY_GRAD 8u
 
 typedef struct rfb_pipeline rfb_pipeline;
 
@@ -206,6 +213,19 @@ int rfb_trace_backward_accumulate(
     const uint32_t *quantile_point_indices, const void *ray_rgba,
     const void *ray_rgba_grad, const float *depth_grad, const void *ray_error,
     void *point_error, const rfb_launch_opts *opts, void *stream);
+/* rfb_trace_backward_accumulate that also writes ray_grad[R][6] (see RFB_FLAG_RAY_GRAD; NULL = not wanted,
+ * which is rfb_trace_backward_accumulate).  RFB_FLAG_SCRUB_NONFINITE in opts->flags zeroes its non-finite
+ * entries; the accumulator itself is never scrubbed (finalize does that). */
+int rfb_trace_backward_accumulate_rays(
+    rfb_pipeline *pipeline, const rfb_trace_settings *settings,
+    uint32_t num_points, const float *points, const void *attributes,
+    uint32_t point_adjacency_size, const uint32_t *point_adjacency,
+    const uint32_t *point_adjacency_offsets, uint32_t num_rays,
+    const float *rays, const uint32_t *start_point_index,
+    uint32_t num_depth_quantiles, const float *depth_quantiles,
+    const uint32_t *quantile_point_indices, const void *ray_rgba,
+    const void *ray_rgba_grad, const float *depth_grad, const void *ray_error,
+    void *point_error, float *ray_grad, const rfb_launch_opts *opts, void *stream);
 /* device pointer + element count of the fp32 accumulator of the last accumulate */
 int rfb_grad_accumulator(rfb_pipeline *pipeline, float **ptr, uint64_t *num_floats);
 uint32_t rfb_grad_row_floats(const rfb_pipeline *pipeline);

@@ -43,6 +43,7 @@ class LaunchOpts(ctypes.Structure):  # rfb_launch_opts
 FLAG_SCRUB_NONFINITE = 1
 FLAG_RECORD_TAPE = 2
 FLAG_USE_TAPE = 4
+FLAG_RAY_GRAD = 8
 
 # name -> (restype, argtypes); must list every symbol include/radfoam_b200.h declares
 _P = c_void_p
@@ -66,6 +67,9 @@ SIGNATURES = {
     "rfb_trace_backward_accumulate": (c_int, [_P, POINTER(TraceSettings), c_uint32, _P, _P, c_uint32,
                                               _P, _P, c_uint32, _P, _P, c_uint32, _P, _P, _P, _P, _P,
                                               _P, _P, POINTER(LaunchOpts), _P]),
+    "rfb_trace_backward_accumulate_rays": (c_int, [_P, POINTER(TraceSettings), c_uint32, _P, _P, c_uint32,
+                                                   _P, _P, c_uint32, _P, _P, c_uint32, _P, _P, _P, _P, _P,
+                                                   _P, _P, _P, POINTER(LaunchOpts), _P]),
     "rfb_grad_accumulator": (c_int, [_P, POINTER(_P), POINTER(c_uint64)]),
     "rfb_grad_row_floats": (c_uint32, [_P]),
     "rfb_trace_backward_finalize": (c_int, [_P, c_uint32, _P, _P, c_uint32, _P]),

@@ -436,15 +436,18 @@ __device__ __forceinline__ void isect_grad(float px, float py, float pz, float q
 // commutes with rounding) and leaves a and dp*dp unchanged, so the second gradient reuses them:
 //   gq_i = -( fma(num, d_i, dp * (o_i - q_i)) / (dp*dp) )
 // bit-identical to isect_grad(q, p, ...), at roughly half its cost.
+// The plane's n = q - p, dp = n.d and num = ((p + q)/2 - o).n are returned as well (the ray gradient's
+// dt/do = -n/dp and dt/dd = -(num/dp) n/dp reuse them).
 __device__ __forceinline__ void isect_grad_pair(float px, float py, float pz, float qx, float qy,
                                                 float qz, const RayGeom &ray, float &gpx, float &gpy,
-                                                float &gpz, float &gqx, float &gqy, float &gqz) {
-    float nx = __fsub_rn(qx, px), ny = __fsub_rn(qy, py), nz = __fsub_rn(qz, pz);
+                                                float &gpz, float &gqx, float &gqy, float &gqz, float &nx,
+                                                float &ny, float &nz, float &dp, float &num) {
+    nx = __fsub_rn(qx, px), ny = __fsub_rn(qy, py), nz = __fsub_rn(qz, pz);
     float ax = __fmaf_rn(__fadd_rn(px, qx), 0.5f, -ray.ox);
     float ay = __fmaf_rn(__fadd_rn(py, qy), 0.5f, -ray.oy);
     float az = __fmaf_rn(__fadd_rn(pz, qz), 0.5f, -ray.oz);
-    float dp = __fmaf_rn(nx, ray.dx, __fmaf_rn(ny, ray.dy, __fmul_rn(nz, ray.dz)));
-    float num = __fmaf_rn(nx, ax, __fmaf_rn(ny, ay, __fmul_rn(nz, az)));
+    dp = __fmaf_rn(nx, ray.dx, __fmaf_rn(ny, ray.dy, __fmul_rn(nz, ray.dz)));
+    num = __fmaf_rn(nx, ax, __fmaf_rn(ny, ay, __fmul_rn(nz, az)));
     float inv = __fmul_rn(dp, dp);
     gpx = __fdiv_rn(__fmaf_rn(num, ray.dx, __fmul_rn(dp, __fsub_rn(ray.ox, px))), inv);
     gpy = __fdiv_rn(__fmaf_rn(num, ray.dy, __fmul_rn(dp, __fsub_rn(ray.oy, py))), inv);
@@ -452,6 +455,122 @@ __device__ __forceinline__ void isect_grad_pair(float px, float py, float pz, fl
     gqx = -__fdiv_rn(__fmaf_rn(num, ray.dx, __fmul_rn(dp, __fsub_rn(ray.ox, qx))), inv);
     gqy = -__fdiv_rn(__fmaf_rn(num, ray.dy, __fmul_rn(dp, __fsub_rn(ray.oy, qy))), inv);
     gqz = -__fdiv_rn(__fmaf_rn(num, ray.dz, __fmul_rn(dp, __fsub_rn(ray.oz, qz))), inv);
+}
+
+// Per-ray sums of the ray gradient dL/d(origin, direction) (the RAY instantiations of the backward kernels;
+// DESIGN.md §2).  The walk's cell sequence is held fixed: a composited cell's t1 lies on its exit plane
+// (cur, next) and its t0 on the exit plane of the previous composited cell, both planes of the fp32 points, with
+// dt/do = -n/dp and dt/dd = -(num/dp) n/dp (d the unit direction).  The colour's dependence on the direction
+// is summed separately, as G_k = sum over cells and channels of dL/drgb_c * a[cell, 3k+c] (ray_grad_store()).
+struct RayAcc {
+    float gox, goy, goz; // dL/do
+    float gdx, gdy, gdz; // dL/dd (unit direction) through the planes
+    float jx, jy, jz;    // exit plane of the previous composited cell: -n/dp ...
+    float jt;            // ... and num/dp
+    __device__ __forceinline__ void init() {
+        gox = goy = goz = gdx = gdy = gdz = 0.0f;
+        jx = jy = jz = jt = 0.0f;
+    }
+    // dL/dt * (dt/do, dt/dd) of the plane (jx, jy, jz, jt)
+    __device__ __forceinline__ void add(float dL_dt, float px, float py, float pz, float pt) {
+        gox = __fmaf_rn(dL_dt, px, gox);
+        goy = __fmaf_rn(dL_dt, py, goy);
+        goz = __fmaf_rn(dL_dt, pz, goz);
+        const float s = __fmul_rn(dL_dt, pt);
+        gdx = __fmaf_rn(s, px, gdx);
+        gdy = __fmaf_rn(s, py, gdy);
+        gdz = __fmaf_rn(s, pz, gdz);
+    }
+};
+
+// G_k += sum_c dL/drgb_c * a[3k+c] for one cell's SH row (the row sh_to_rgb read; L1-resident by now)
+template <int DEG>
+__device__ __forceinline__ void sh_grad_contract(const float *__restrict__ row, const float dL_drgb[3],
+                                                 float *G) {
+    if (dL_drgb[0] == 0.0f && dL_drgb[1] == 0.0f && dL_drgb[2] == 0.0f)
+        return;
+    constexpr int NV = sh_row(DEG) / 4;
+    float v[NV * 4];
+    const float4 *row4 = reinterpret_cast<const float4 *>(row);
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+        float4 q = ldg4(row4 + i);
+        v[4 * i + 0] = q.x;
+        v[4 * i + 1] = q.y;
+        v[4 * i + 2] = q.z;
+        v[4 * i + 3] = q.w;
+    }
+#pragma unroll
+    for (int k = 0; k < sh_dim(DEG); ++k)
+        G[k] = __fmaf_rn(dL_drgb[2], v[3 * k + 2],
+                         __fmaf_rn(dL_drgb[1], v[3 * k + 1], __fmaf_rn(dL_drgb[0], v[3 * k], G[k])));
+}
+
+// (gx, gy, gz) += sum_k G_k grad Y_k(x, y, z): the gradient of the real SH basis of sh_basis() (same constants).
+// Every operation is an explicit intrinsic, so that all kernels that inline this round it the same way (ray_grad
+// is bit-identical across the direct, re-walk and replay backward).
+template <int DEG>
+__device__ __forceinline__ void sh_basis_grad(float x, float y, float z, const float *G, float &gx, float &gy,
+                                              float &gz) {
+    // g += c * m
+    auto acc = [](float &g, float c, float m) { g = __fmaf_rn(c, m, g); };
+    constexpr float C1 = 0.4886025119029199f;
+    if (DEG > 0) {
+        acc(gy, -C1, G[1]);
+        acc(gz, C1, G[2]);
+        acc(gx, -C1, G[3]);
+    }
+    if (DEG > 1) {
+        // Y4 = A xy, Y5 = -A yz, Y6 = B (2zz - xx - yy), Y7 = -A xz, Y8 = C (xx - yy)
+        constexpr float A = 1.0925484305920792f, B2 = 2.0f * 0.31539156525252005f, C2 = 2.0f * 0.5462742152960396f;
+        const float g4 = __fmul_rn(A, G[4]), g5 = __fmul_rn(A, G[5]), g6 = __fmul_rn(B2, G[6]),
+                    g7 = __fmul_rn(A, G[7]), g8 = __fmul_rn(C2, G[8]);
+        acc(gx, g4, y);
+        acc(gy, g4, x);
+        acc(gy, -g5, z);
+        acc(gz, -g5, y);
+        acc(gx, -g6, x);
+        acc(gy, -g6, y);
+        acc(gz, __fmul_rn(2.0f, g6), z);
+        acc(gx, -g7, z);
+        acc(gz, -g7, x);
+        acc(gx, g8, x);
+        acc(gy, -g8, y);
+    }
+    if (DEG > 2) {
+        const float xx = __fmul_rn(x, x), yy = __fmul_rn(y, y), zz = __fmul_rn(z, z);
+        const float xy = __fmul_rn(x, y), yz = __fmul_rn(y, z), xz = __fmul_rn(x, z);
+        const float g9 = __fmul_rn(-0.5900435899266435f, G[9]), g10 = __fmul_rn(2.890611442640554f, G[10]),
+                    g11 = __fmul_rn(-0.4570457994644658f, G[11]), g12 = __fmul_rn(0.3731763325901154f, G[12]),
+                    g13 = __fmul_rn(-0.4570457994644658f, G[13]), g14 = __fmul_rn(1.445305721320277f, G[14]),
+                    g15 = __fmul_rn(-0.5900435899266435f, G[15]);
+        // Y9 = c9 y (3xx - yy)
+        acc(gx, __fmul_rn(6.0f, g9), xy);
+        acc(gy, __fmul_rn(3.0f, g9), __fsub_rn(xx, yy));
+        // Y10 = c10 xyz
+        acc(gx, g10, yz);
+        acc(gy, g10, xz);
+        acc(gz, g10, xy);
+        // Y11 = c11 y (4zz - xx - yy)
+        acc(gx, __fmul_rn(-2.0f, g11), xy);
+        acc(gy, g11, __fsub_rn(__fsub_rn(__fmul_rn(4.0f, zz), xx), __fmul_rn(3.0f, yy)));
+        acc(gz, __fmul_rn(8.0f, g11), yz);
+        // Y12 = c12 z (2zz - 3xx - 3yy)
+        acc(gx, __fmul_rn(-6.0f, g12), xz);
+        acc(gy, __fmul_rn(-6.0f, g12), yz);
+        acc(gz, __fmul_rn(3.0f, g12), __fsub_rn(__fsub_rn(__fmul_rn(2.0f, zz), xx), yy));
+        // Y13 = c13 x (4zz - xx - yy)
+        acc(gx, g13, __fsub_rn(__fsub_rn(__fmul_rn(4.0f, zz), __fmul_rn(3.0f, xx)), yy));
+        acc(gy, __fmul_rn(-2.0f, g13), xy);
+        acc(gz, __fmul_rn(8.0f, g13), xz);
+        // Y14 = c14 z (xx - yy)
+        acc(gx, __fmul_rn(2.0f, g14), xz);
+        acc(gy, __fmul_rn(-2.0f, g14), yz);
+        acc(gz, g14, __fsub_rn(xx, yy));
+        // Y15 = c15 x (xx - 3yy)
+        acc(gx, __fmul_rn(3.0f, g15), __fsub_rn(xx, yy));
+        acc(gy, __fmul_rn(-6.0f, g15), xy);
+    }
 }
 
 // Per-ray state of the backward pass and the analytic gradients of one composited cell
@@ -487,12 +606,13 @@ struct BackwardRay {
     // Gradients of one cell.  Outputs: dL/drgb (ReLU-masked), dL/dsigma, and -- when
     // `flush` -- the finished position gradient (fx,fy,fz) of point `flush_idx` (the
     // previous composited cell: gradients are flushed one cell late, quirk A.5.1).
-    // Returns whether the ray continues.
+    // Returns whether the ray continues.  RAY: also adds the cell's plane terms of the ray gradient to `ra`.
+    template <bool RAY>
     __device__ __forceinline__ bool cell(uint32_t cur, const float4 &pc, const float4 &pn,
                                          float t0, float t1, const float rgb[3],
                                          const RayGeom &ray, float weight_threshold,
                                          float dL_drgb[3], float &dL_ds, float &w_out, bool &flush,
-                                         uint32_t &flush_idx, float &fx_, float &fy_, float &fz_) {
+                                         uint32_t &flush_idx, float &fx_, float &fy_, float &fz_, RayAcc &ra) {
         const float s = pc.w;
         float delta = fmaxf(__fsub_rn(t1, t0), 0.0f);
         float alpha = 1.0f - expf(__fmul_rn(s, -delta));
@@ -514,8 +634,12 @@ struct BackwardRay {
         float Tn = __fmul_rn(oma, T);
         dL_ds = __fmul_rn(dL_dalpha, __fmul_rn(delta, oma));
         float dL_dt0 = 0.0f;
+        float ray_dt0 = 0.0f; // RAY: sum of the depth gradients of the quantiles this cell fires (d depth / d t0 = 1)
         while (qi < Q && Tn < cq) {
-            float gq = __fdiv_rn(__ldg(dg + qi), s);
+            const float dgq = __ldg(dg + qi);
+            if (RAY)
+                ray_dt0 = __fadd_rn(ray_dt0, dgq);
+            float gq = __fdiv_rn(dgq, s);
             dL_dt0 = __fadd_rn(gq, dL_dt0);
             float m = __fmul_rn(logf(__fdiv_rn(T, cq)), gq);
             dL_ds = __fsub_rn(dL_ds, __fdiv_rn(m, s));
@@ -537,10 +661,22 @@ struct BackwardRay {
         // entry plane (prev | cur): e = dt0/dcur, a = dt0/dprev; exit plane (cur | next):
         // b = dt1/dcur, n = dt1/dnext.  Before the first composited cell prev_point is the
         // origin (quirk A.5.2) and dt0/dprev is defined as zero (pipeline.cu:284-289).
-        isect_grad_pair(pc.x, pc.y, pc.z, ppx, ppy, ppz, ray, ex, ey, ez, ax, ay, az);
+        float pnx, pny, pnz, pdp, pnum; // planes (cur | prev) and (cur | next)
+        isect_grad_pair(pc.x, pc.y, pc.z, ppx, ppy, ppz, ray, ex, ey, ez, ax, ay, az, pnx, pny, pnz, pdp, pnum);
         if (prev == kNone)
             ax = ay = az = 0.0f;
-        isect_grad_pair(pc.x, pc.y, pc.z, pn.x, pn.y, pn.z, ray, bx, by, bz, nx, ny, nz);
+        isect_grad_pair(pc.x, pc.y, pc.z, pn.x, pn.y, pn.z, ray, bx, by, bz, nx, ny, nz, pnx, pny, pnz, pdp, pnum);
+        if (RAY) {
+            // t0 lies on the previous composited cell's exit plane (the constant 0 before the first one), t1 on
+            // this cell's; dL/dt0 takes the depth gradients themselves, not the point gradient's gd / sigma
+            if (prev != kNone)
+                ra.add(__fsub_rn(ray_dt0, dL_dd), ra.jx, ra.jy, ra.jz, ra.jt);
+            ra.jx = -__fdiv_rn(pnx, pdp);
+            ra.jy = -__fdiv_rn(pny, pdp);
+            ra.jz = -__fdiv_rn(pnz, pdp);
+            ra.jt = __fdiv_rn(pnum, pdp);
+            ra.add(dL_dt1, ra.jx, ra.jy, ra.jz, ra.jt);
+        }
         pgx = __fmaf_rn(dL_dt0, ax, pgx);
         pgy = __fmaf_rn(dL_dt0, ay, pgy);
         pgz = __fmaf_rn(dL_dt0, az, pgz);

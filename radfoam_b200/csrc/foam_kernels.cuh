@@ -677,6 +677,34 @@ __device__ __forceinline__ void backward_ray_setup(const BackwardParams &p, uint
     }
 }
 
+// Output of the RAY instantiations of the backward kernels: ray_grad[R][6] = dL/d(origin, direction as passed
+// in), every ray written (no atomics).  A separate, trailing kernel parameter so that BackwardParams and the
+// parameters after it keep their layout in the default instantiations.
+struct RayGradOut {
+    float *ray_grad;
+    int scrub; // zero non-finite entries
+};
+
+// ray_grad[r] from the walk's sums: the colour's direction term sum_k G_k grad Y_k(d) is added, and the unit
+// direction's gradient g is taken back through d = d_in / |d_in|: (g - d (d.g)) / |d_in|, with |d_in| the fp32
+// norm normalize_dir() divides by
+template <int DEG>
+__device__ __forceinline__ void ray_grad_store(const BackwardParams &p, const RayGradOut &rg, uint32_t r,
+                                               const RayGeom &ray, const RayAcc &ra, const float *G) {
+    float gx = ra.gdx, gy = ra.gdy, gz = ra.gdz;
+    sh_basis_grad<DEG>(ray.dx, ray.dy, ray.dz, G, gx, gy, gz);
+    const float *rp = p.rays + 6 * (uint64_t)r;
+    const float x = __ldg(rp + 3), y = __ldg(rp + 4), z = __ldg(rp + 5);
+    const float norm = __fsqrt_rn(__fmaf_rn(x, x, __fmaf_rn(y, y, __fmul_rn(z, z))));
+    const float dg = __fmaf_rn(ray.dx, gx, __fmaf_rn(ray.dy, gy, __fmul_rn(ray.dz, gz)));
+    float v[6] = {ra.gox, ra.goy, ra.goz, __fdiv_rn(__fmaf_rn(-ray.dx, dg, gx), norm),
+                  __fdiv_rn(__fmaf_rn(-ray.dy, dg, gy), norm), __fdiv_rn(__fmaf_rn(-ray.dz, dg, gz), norm)};
+    float *out = rg.ray_grad + 6 * (uint64_t)r;
+#pragma unroll
+    for (int i = 0; i < 6; ++i)
+        out[i] = (rg.scrub && !isfinite(v[i])) ? 0.0f : v[i];
+}
+
 __device__ __forceinline__ void add_point_error(const BackwardParams &p, uint32_t cell, float v) {
     if (p.io_half)
         atomicAdd(reinterpret_cast<__half *>(p.point_error) + cell, __float2half_rn(v));
@@ -704,8 +732,10 @@ __device__ __forceinline__ void reduce_row_direct(float *row, const float *sh, c
 }
 
 // ---- backward, direct: every lane reduces its own rows straight to HBM
-template <int DEG, typename Faces>
-__global__ void __launch_bounds__(kBlock) backward_kernel(const BackwardParams p, const Faces fa) {
+// RAY: also writes ray_grad (RayGradOut)
+template <int DEG, typename Faces, bool RAY>
+__global__ void __launch_bounds__(kBlock) backward_kernel(const BackwardParams p, const Faces fa,
+                                                          const RayGradOut rg) {
     uint32_t r;
     if (!thread_ray(p.num_rays, p.image_width, p.blocks_x, r))
         return;
@@ -715,6 +745,14 @@ __global__ void __launch_bounds__(kBlock) backward_kernel(const BackwardParams p
     float sh[sh_dim(DEG)];
     BackwardRay st;
     backward_ray_setup<DEG>(p, r, ray, sh, st);
+    RayAcc ra;
+    float G[sh_dim(DEG)];
+    if (RAY) {
+        ra.init();
+#pragma unroll
+        for (int k = 0; k < sh_dim(DEG); ++k)
+            G[k] = 0.0f;
+    }
 
     auto cell_fn = [&](uint32_t cell, const float4 &pc, float t0, float t1, const float4 &pn) -> bool {
         float rgb[3] = {0.0f, 0.0f, 0.0f};
@@ -723,8 +761,10 @@ __global__ void __launch_bounds__(kBlock) backward_kernel(const BackwardParams p
         float dL_drgb[3], dL_ds, w, fx, fy, fz;
         bool flush;
         uint32_t flush_idx;
-        bool go = st.cell(cell, pc, pn, t0, t1, rgb, ray, p.weight_threshold, dL_drgb, dL_ds, w, flush,
-                          flush_idx, fx, fy, fz);
+        bool go = st.template cell<RAY>(cell, pc, pn, t0, t1, rgb, ray, p.weight_threshold, dL_drgb, dL_ds, w,
+                                        flush, flush_idx, fx, fy, fz, ra);
+        if (RAY)
+            sh_grad_contract<DEG>(p.sh_rows + (uint64_t)cell * SR, dL_drgb, G);
         if (p.point_error)
             add_point_error(p, cell, __fmul_rn(w, st.err));
         if (flush)
@@ -733,6 +773,8 @@ __global__ void __launch_bounds__(kBlock) backward_kernel(const BackwardParams p
         return go;
     };
     walk(fa, p.cells, ray, __ldg(p.start + r), p.max_steps, cell_fn);
+    if (RAY)
+        ray_grad_store<DEG>(p, rg, r, ray, ra, G);
 }
 
 // ---- backward, warp-aggregated
@@ -758,9 +800,10 @@ __global__ void __launch_bounds__(kBlock) backward_kernel(const BackwardParams p
 // at the tape's overflow flag first and exactly one of them does the work (the other returns at
 // once), so a pool overflow needs no host round trip.  (Prefetching the next cell's SH row into
 // L1 or L2 as soon as the cell is known was tried and is no faster.)
-template <int DEG, typename Faces, int SLOTS, int MIN_GROUP, int MIN_BLOCKS, bool REPLAY>
+// RAY: also writes ray_grad (RayGradOut), in both the replay and the re-walk instantiation.
+template <int DEG, typename Faces, int SLOTS, int MIN_GROUP, int MIN_BLOCKS, bool REPLAY, bool RAY>
 __global__ void __launch_bounds__(kBlock, MIN_BLOCKS * 128 / kBlock)
-    backward_cached_kernel(const BackwardParams p, const Faces fa, const Tape tape) {
+    backward_cached_kernel(const BackwardParams p, const Faces fa, const Tape tape, const RayGradOut rg) {
     if (tape.pool != nullptr) {
         const bool overflowed = tape.ctrl[1] != 0u;
         if (REPLAY == overflowed) // replay kernel on an overflowed tape / re-walk kernel on a good one
@@ -791,6 +834,7 @@ __global__ void __launch_bounds__(kBlock, MIN_BLOCKS * 128 / kBlock)
     const uint32_t tile = (replay && tape.order) ? tape.order[blockIdx.x] : blockIdx.x; // longest tiles first
     uint32_t r;
     bool done = !thread_ray(p.num_rays, p.image_width, p.blocks_x, r, tile);
+    const bool has_ray = !done;
     RayGeom ray = {0.f, 0.f, 0.f, 0.f, 0.f, 1.f};
     float sh[sh_dim(DEG)];
     BackwardRay st;
@@ -832,6 +876,15 @@ __global__ void __launch_bounds__(kBlock, MIN_BLOCKS * 128 / kBlock)
             rec = tape_row(chunk_ahead, 0);
             recB = tape_row(chunk_ahead, 1);
         }
+    }
+
+    RayAcc ra;
+    float G[sh_dim(DEG)];
+    if (RAY) {
+        ra.init();
+#pragma unroll
+        for (int k = 0; k < sh_dim(DEG); ++k)
+            G[k] = 0.0f;
     }
 
     for (uint32_t k = 0;; ++k) {
@@ -884,8 +937,10 @@ __global__ void __launch_bounds__(kBlock, MIN_BLOCKS * 128 / kBlock)
                 float w, fx, fy, fz;
                 bool flush;
                 uint32_t flush_idx;
-                bool go = st.cell(cur, pc, pn, t0, t1, rgb, ray, p.weight_threshold, dL_drgb, dL_ds, w,
-                                  flush, flush_idx, fx, fy, fz);
+                bool go = st.template cell<RAY>(cur, pc, pn, t0, t1, rgb, ray, p.weight_threshold, dL_drgb,
+                                                dL_ds, w, flush, flush_idx, fx, fy, fz, ra);
+                if (RAY)
+                    sh_grad_contract<DEG>(p.sh_rows + (uint64_t)cur * SR, dL_drgb, G);
                 if (p.point_error)
                     add_point_error(p, cur, __fmul_rn(w, st.err));
                 if (flush)
@@ -988,6 +1043,8 @@ __global__ void __launch_bounds__(kBlock, MIN_BLOCKS * 128 / kBlock)
             red_add_v4(p.acc + (uint64_t)tag * GR + 4 * lane, v.x, v.y, v.z, v.w);
         }
     }
+    if (RAY && has_ray)
+        ray_grad_store<DEG>(p, rg, r, ray, ra, G);
 }
 
 // accumulator -> reference-layout gradient outputs (+ optional finite scrub): flat over the output elements

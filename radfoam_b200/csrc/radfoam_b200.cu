@@ -452,25 +452,32 @@ int prepare_tape(rfb_pipeline *p, uint32_t blocks, uint32_t num_rays, uint32_t m
     return 0;
 }
 
-template <typename Faces>
-int launch_backward(int deg, const BackwardParams &bp, const Faces &fa, uint32_t blocks,
-                    cudaStream_t stream) {
+template <typename Faces, bool RAY>
+int launch_backward_ray(int deg, const BackwardParams &bp, const Faces &fa, const RayGradOut &rg, uint32_t blocks,
+                        cudaStream_t stream) {
     switch (deg) {
-    case 0: RFB_LAUNCH((backward_kernel<0, Faces>), blocks, kBlock, 0, stream, bp, fa); break;
-    case 1: RFB_LAUNCH((backward_kernel<1, Faces>), blocks, kBlock, 0, stream, bp, fa); break;
-    case 2: RFB_LAUNCH((backward_kernel<2, Faces>), blocks, kBlock, 0, stream, bp, fa); break;
-    default: RFB_LAUNCH((backward_kernel<3, Faces>), blocks, kBlock, 0, stream, bp, fa); break;
+    case 0: RFB_LAUNCH((backward_kernel<0, Faces, RAY>), blocks, kBlock, 0, stream, bp, fa, rg); break;
+    case 1: RFB_LAUNCH((backward_kernel<1, Faces, RAY>), blocks, kBlock, 0, stream, bp, fa, rg); break;
+    case 2: RFB_LAUNCH((backward_kernel<2, Faces, RAY>), blocks, kBlock, 0, stream, bp, fa, rg); break;
+    default: RFB_LAUNCH((backward_kernel<3, Faces, RAY>), blocks, kBlock, 0, stream, bp, fa, rg); break;
     }
     RFB_LAUNCHED();
     return 0;
 }
 
-template <int DEG, typename Faces, int SLOTS, int MIN_GROUP, int MIN_BLOCKS, bool REPLAY>
-int launch_backward_cached_one(const BackwardParams &bp, const Faces &fa, const Tape &tape,
+template <typename Faces>
+int launch_backward(int deg, const BackwardParams &bp, const Faces &fa, const RayGradOut &rg, uint32_t blocks,
+                    cudaStream_t stream) {
+    return rg.ray_grad ? launch_backward_ray<Faces, true>(deg, bp, fa, rg, blocks, stream)
+                       : launch_backward_ray<Faces, false>(deg, bp, fa, rg, blocks, stream);
+}
+
+template <int DEG, typename Faces, int SLOTS, int MIN_GROUP, int MIN_BLOCKS, bool REPLAY, bool RAY>
+int launch_backward_cached_one(const BackwardParams &bp, const Faces &fa, const Tape &tape, const RayGradOut &rg,
                                uint32_t blocks, cudaStream_t stream) {
     constexpr int GR = grad_row(DEG);
     constexpr size_t smem = (size_t)(kBlock / 32) * ((32 * GR + SLOTS * GR + SLOTS + 3) & ~3) * sizeof(float);
-    auto kernel = backward_cached_kernel<DEG, Faces, SLOTS, MIN_GROUP, MIN_BLOCKS, REPLAY>;
+    auto kernel = backward_cached_kernel<DEG, Faces, SLOTS, MIN_GROUP, MIN_BLOCKS, REPLAY, RAY>;
     // the attribute is per device and idempotent: set it once per (instantiation, device)
     static std::atomic<uint64_t> configured{0};
     int dev = 0;
@@ -480,37 +487,49 @@ int launch_backward_cached_one(const BackwardParams &bp, const Faces &fa, const 
         RFB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         configured.fetch_or(bit, std::memory_order_relaxed);
     }
-    RFB_LAUNCH((kernel), blocks, kBlock, smem, stream, bp, fa, tape);
+    RFB_LAUNCH((kernel), blocks, kBlock, smem, stream, bp, fa, tape, rg);
     RFB_LAUNCHED();
     return 0;
 }
 
 // With a tape: the replay kernel and the re-walk kernel are both launched; the tape's overflow
 // flag (device side) decides which one works.  Without: the re-walk kernel alone.
-template <int DEG, typename Faces, int SLOTS, int MIN_GROUP, int MIN_BLOCKS>
-int launch_backward_cached_cfg(const BackwardParams &bp, const Faces &fa, const Tape &tape,
+template <int DEG, typename Faces, int SLOTS, int MIN_GROUP, int MIN_BLOCKS, bool RAY>
+int launch_backward_cached_cfg(const BackwardParams &bp, const Faces &fa, const Tape &tape, const RayGradOut &rg,
                                uint32_t blocks, cudaStream_t stream) {
     if (tape.pool)
-        if (int rc = launch_backward_cached_one<DEG, Faces, SLOTS, MIN_GROUP, MIN_BLOCKS, true>(
-                bp, fa, tape, blocks, stream))
+        if (int rc = launch_backward_cached_one<DEG, Faces, SLOTS, MIN_GROUP, MIN_BLOCKS, true, RAY>(
+                bp, fa, tape, rg, blocks, stream))
             return rc;
-    return launch_backward_cached_one<DEG, Faces, SLOTS, MIN_GROUP, MIN_BLOCKS, false>(bp, fa, tape, blocks,
-                                                                                     stream);
+    return launch_backward_cached_one<DEG, Faces, SLOTS, MIN_GROUP, MIN_BLOCKS, false, RAY>(bp, fa, tape, rg,
+                                                                                          blocks, stream);
 }
 
 // Shipped configuration: 4 cache slots per warp, groups of >= 6 lanes go through the cache, 5 CTAs/SM
 // (<= 102 registers; the H100's 64 K registers per SM hold 5 CTAs of 128 threads at 96).  Fewer slots keep the
 // per-warp staging small; 6 CTAs/SM would spill.  With 4 slots a CTA needs under 32 KB of shared memory, so 5 CTAs
 // take about 150 KB of the H100's 228 KB per SM and the rest stays L1.
+// With ray gradients (RAY) each thread also keeps its ray's sums (the G_k alone are (deg+1)^2 registers): those
+// instantiations get fewer CTAs/SM, so that they do not spill -- 4 (<= 128 registers) for degrees 0-2 and 3
+// (<= 168) for degree 3, which spills at 128.
+template <int DEG, bool RAY>
+constexpr int backward_min_blocks() { return !RAY ? 5 : DEG == 3 ? 3 : 4; }
+template <typename Faces, bool RAY>
+int launch_backward_cached_ray(int deg, const BackwardParams &bp, const Faces &fa, const Tape &tape,
+                               const RayGradOut &rg, uint32_t blocks, cudaStream_t stream) {
+    switch (deg) {
+    case 0: return launch_backward_cached_cfg<0, Faces, 4, 6, backward_min_blocks<0, RAY>(), RAY>(bp, fa, tape, rg, blocks, stream);
+    case 1: return launch_backward_cached_cfg<1, Faces, 4, 6, backward_min_blocks<1, RAY>(), RAY>(bp, fa, tape, rg, blocks, stream);
+    case 2: return launch_backward_cached_cfg<2, Faces, 4, 6, backward_min_blocks<2, RAY>(), RAY>(bp, fa, tape, rg, blocks, stream);
+    default: return launch_backward_cached_cfg<3, Faces, 4, 6, backward_min_blocks<3, RAY>(), RAY>(bp, fa, tape, rg, blocks, stream);
+    }
+}
+
 template <typename Faces>
 int launch_backward_cached(int deg, const BackwardParams &bp, const Faces &fa, const Tape &tape,
-                           uint32_t blocks, cudaStream_t stream) {
-    switch (deg) {
-    case 0: return launch_backward_cached_cfg<0, Faces, 4, 6, 5>(bp, fa, tape, blocks, stream);
-    case 1: return launch_backward_cached_cfg<1, Faces, 4, 6, 5>(bp, fa, tape, blocks, stream);
-    case 2: return launch_backward_cached_cfg<2, Faces, 4, 6, 5>(bp, fa, tape, blocks, stream);
-    default: return launch_backward_cached_cfg<3, Faces, 4, 6, 5>(bp, fa, tape, blocks, stream);
-    }
+                           const RayGradOut &rg, uint32_t blocks, cudaStream_t stream) {
+    return rg.ray_grad ? launch_backward_cached_ray<Faces, true>(deg, bp, fa, tape, rg, blocks, stream)
+                       : launch_backward_cached_ray<Faces, false>(deg, bp, fa, tape, rg, blocks, stream);
 }
 
 template <typename Faces, int MODE>
@@ -862,7 +881,24 @@ int rfb_trace_backward_accumulate(rfb_pipeline *p, const rfb_trace_settings *set
                                   const uint32_t *quantile_point_indices, const void *ray_rgba,
                                   const void *ray_rgba_grad, const float *depth_grad,
                                   const void *ray_error, void *point_error,
-                                  const rfb_launch_opts *opts, void *stream_) {
+                                  const rfb_launch_opts *opts, void *stream) {
+    return rfb_trace_backward_accumulate_rays(p, settings, num_points, points, attributes, point_adjacency_size,
+                                              point_adjacency, point_adjacency_offsets, num_rays, rays,
+                                              start_point_index, num_depth_quantiles, depth_quantiles,
+                                              quantile_point_indices, ray_rgba, ray_rgba_grad, depth_grad, ray_error,
+                                              point_error, nullptr, opts, stream);
+}
+
+int rfb_trace_backward_accumulate_rays(rfb_pipeline *p, const rfb_trace_settings *settings,
+                                       uint32_t num_points, const float *points, const void *attributes,
+                                       uint32_t point_adjacency_size, const uint32_t *point_adjacency,
+                                       const uint32_t *point_adjacency_offsets, uint32_t num_rays,
+                                       const float *rays, const uint32_t *start_point_index,
+                                       uint32_t num_depth_quantiles, const float *depth_quantiles,
+                                       const uint32_t *quantile_point_indices, const void *ray_rgba,
+                                       const void *ray_rgba_grad, const float *depth_grad,
+                                       const void *ray_error, void *point_error, float *ray_grad,
+                                       const rfb_launch_opts *opts, void *stream_) {
     if (!p)
         return fail("rfb_trace_backward: pipeline is NULL");
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -940,8 +976,11 @@ int rfb_trace_backward_accumulate(rfb_pipeline *p, const rfb_trace_settings *set
         if (int rc = wait_for(p->tape_ready, p->tape_stream, stream))
             return rc;
     }
-    if (int rc = cached ? launch_backward_cached(p->sh_degree, bp, fa, tape, blocks, stream)
-                        : launch_backward(p->sh_degree, bp, fa, blocks, stream))
+    RayGradOut rg;
+    rg.ray_grad = ray_grad;
+    rg.scrub = (opts && (opts->flags & RFB_FLAG_SCRUB_NONFINITE)) ? 1 : 0;
+    if (int rc = cached ? launch_backward_cached(p->sh_degree, bp, fa, tape, rg, blocks, stream)
+                        : launch_backward(p->sh_degree, bp, fa, rg, blocks, stream))
         return rc;
     return profile_mark(p, 3, stream);
 }
@@ -1138,15 +1177,18 @@ int rfb_trace_backward(rfb_pipeline *p, const rfb_trace_settings *settings, uint
                        const void *ray_rgba_grad, const float *depth_grad, const void *ray_error,
                        float *ray_grad, float *points_grad, void *attribute_grad, void *point_error,
                        const rfb_launch_opts *opts, void *stream) {
-    (void)ray_grad; // never written, like the reference kernel (SURVEY.md A.5 quirk 4)
     if (p && p->params_bound)
         return fail("rfb_trace_backward: a parameter-form scene is bound; use rfb_trace_backward_accumulate + "
                     "rfb_trace_backward_finalize_params");
-    if (int rc = rfb_trace_backward_accumulate(
+    // without RFB_FLAG_RAY_GRAD ray_grad is not written, like the reference kernel (SURVEY.md A.5 quirk 4)
+    const bool want_rays = opts && (opts->flags & RFB_FLAG_RAY_GRAD);
+    if (want_rays && !ray_grad)
+        return fail("rfb_trace_backward: RFB_FLAG_RAY_GRAD is set but ray_grad is NULL");
+    if (int rc = rfb_trace_backward_accumulate_rays(
             p, settings, num_points, points, attributes, point_adjacency_size, point_adjacency,
             point_adjacency_offsets, num_rays, rays, start_point_index, num_depth_quantiles,
             depth_quantiles, quantile_point_indices, ray_rgba, ray_rgba_grad, depth_grad, ray_error,
-            point_error, opts, stream))
+            point_error, want_rays ? ray_grad : nullptr, opts, stream))
         return rc;
     return rfb_trace_backward_finalize(p, num_points, points_grad, attribute_grad,
                                        opts ? opts->flags : 0, stream);

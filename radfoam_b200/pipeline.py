@@ -307,7 +307,9 @@ class Pipeline:
             depth_indices = torch.empty(batch + [num_q], dtype=torch.uint32, device=dev)
 
         trainable = (points, attributes) if attributes is not None else (points,) + self._params[1]
-        record = self.record_tape and self.cache_scene and self._backward_expected(trainable)
+        # through the autograd ops, rays that require grad expect a backward too (ray gradients)
+        rays_grad = bool(self.autograd_recording) and rays.requires_grad
+        record = self.record_tape and self.cache_scene and (self._backward_expected(trainable) or rays_grad)
         opts = self._opts(scene_key, rays_c, _lib.FLAG_RECORD_TAPE if record else 0)
         self._tape_refs = ([(weakref.ref(t), t._version) for t in (rays_c, start_c)]
                            + [opts.scene_version] if record else None)
@@ -345,6 +347,14 @@ class Pipeline:
         del dq_k  # the backward's own quantiles are permuted, whatever the forward was given
         return (rays_k, start_k, take(rgb_c, perm), take(grad_c, perm), take(dq_c, perm),
                 take(di_c, perm), take(dg_c, perm), take(err_c, perm))
+
+    def _caller_order(self, ray_grad, rays_traced, rays_in):
+        """A per-ray backward output in the caller's ray order: _sorted_backward_args may have handed the kernels
+        the forward's coherently sorted copy of the rays instead of ``rays_in``."""
+        if rays_traced is rays_in:
+            return ray_grad
+        with torch.no_grad():
+            return self._untake(ray_grad, self._reorder[2]).view(rays_in.shape)
 
     def _backward_args(self, points, attributes, point_adjacency, point_adjacency_offsets, rays,
                        start_point, rgb_out, grad_in, depth_quantiles, depth_indices,
@@ -424,14 +434,18 @@ class Pipeline:
     def trace_backward(self, points, attributes, point_adjacency, point_adjacency_offsets, rays,
                        start_point, rgb_out, grad_in, depth_quantiles=None, depth_indices=None,
                        depth_grad_in=None, ray_error=None, weight_threshold=None,
-                       max_intersections=None, scrub_nonfinite=False):
+                       max_intersections=None, scrub_nonfinite=False, return_ray_grad=False):
         """``scrub_nonfinite`` (extension, default off) zeroes non-finite gradient
         entries inside the kernel epilogue, saving the two masked passes
-        radfoam_model/render.py:98-99 makes after this call."""
+        radfoam_model/render.py:98-99 makes after this call.  ``return_ray_grad``
+        (extension, default off) fills ``ray_grad`` with dL/d(origin, direction as passed
+        in) for the walk's cell sequence held fixed; otherwise it is allocated and never
+        written, as in the reference."""
         (points_c, attributes_c, adj_c, off_c, rays_c, start_c, rgb_c, grad_c, dq_c, di_c, dg_c,
          err_c, num_rays, num_q) = self._backward_args(
             points, attributes, point_adjacency, point_adjacency_offsets, rays, start_point, rgb_out,
             grad_in, depth_quantiles, depth_indices, depth_grad_in, ray_error)
+        rays_in = rays_c
         with torch.no_grad():
             rays_c, start_c, rgb_c, grad_c, dq_c, di_c, dg_c, err_c = self._sorted_backward_args(
                 rays_c, start_c, rgb_c, grad_c, dq_c, di_c, dg_c, err_c)
@@ -443,12 +457,14 @@ class Pipeline:
             raise RuntimeError("a parameter-form scene is bound: use trace_backward_params")
         attr_grad = torch.empty((num_points, self._attr_dim), dtype=self._dtype, device=dev)
         points_grad = torch.empty((num_points, 3), dtype=torch.float32, device=dev)
-        ray_grad = torch.empty_like(rays_c)  # never written, like the reference (SURVEY A.5.4)
+        # without return_ray_grad never written, like the reference (SURVEY A.5.4)
+        ray_grad = torch.empty_like(rays_c)
         point_error = None
         if err_c is not None:
             point_error = torch.zeros((num_points, 1), dtype=self._dtype, device=dev)
 
-        opts = self._opts(self._scene_key, rays_c, _lib.FLAG_SCRUB_NONFINITE if scrub_nonfinite else 0)
+        flags = (_lib.FLAG_SCRUB_NONFINITE if scrub_nonfinite else 0) | (_lib.FLAG_RAY_GRAD if return_ray_grad else 0)
+        opts = self._opts(self._scene_key, rays_c, flags)
         opts.flags |= self._tape_flag(rays_c, start_c, opts.scene_version)
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream(dev).cuda_stream
@@ -458,6 +474,8 @@ class Pipeline:
                 num_q, _ptr(dq_c), _ptr(di_c), _ptr(rgb_c), _ptr(grad_c), _ptr(dg_c), _ptr(err_c),
                 _ptr(ray_grad), _ptr(points_grad), _ptr(attr_grad), _ptr(point_error),
                 ctypes.byref(opts), stream))
+        if return_ray_grad:
+            ray_grad = self._caller_order(ray_grad, rays_c, rays_in)
 
         out = {"points_grad": points_grad, "attr_grad": attr_grad, "ray_grad": ray_grad}
         if err_c is not None:
@@ -468,14 +486,18 @@ class Pipeline:
     def trace_backward_accumulate(self, points, attributes, point_adjacency,
                                   point_adjacency_offsets, rays, start_point, rgb_out, grad_in,
                                   depth_quantiles=None, depth_indices=None, depth_grad_in=None,
-                                  ray_error=None, weight_threshold=None, max_intersections=None):
+                                  ray_error=None, weight_threshold=None, max_intersections=None,
+                                  return_ray_grad=False, scrub_nonfinite=False):
         """Backward into the pipeline's fp32 accumulator; returns it as a
         ``[N, grad_row_floats]`` tensor VIEW (valid until the next call) so a
-        data-parallel caller can all-reduce it before ``trace_backward_finalize``."""
+        data-parallel caller can all-reduce it before ``trace_backward_finalize``.
+        With ``return_ray_grad`` a third value is returned: ``ray_grad`` (see
+        ``trace_backward``), whose non-finite entries ``scrub_nonfinite`` zeroes."""
         (points_c, attributes_c, adj_c, off_c, rays_c, start_c, rgb_c, grad_c, dq_c, di_c, dg_c,
          err_c, num_rays, num_q) = self._backward_args(
             points, attributes, point_adjacency, point_adjacency_offsets, rays, start_point, rgb_out,
             grad_in, depth_quantiles, depth_indices, depth_grad_in, ray_error)
+        rays_in = rays_c
         with torch.no_grad():
             rays_c, start_c, rgb_c, grad_c, dq_c, di_c, dg_c, err_c = self._sorted_backward_args(
                 rays_c, start_c, rgb_c, grad_c, dq_c, di_c, dg_c, err_c)
@@ -485,16 +507,19 @@ class Pipeline:
         point_error = None
         if err_c is not None:
             point_error = torch.zeros((num_points, 1), dtype=self._dtype, device=dev)
-        opts = self._opts(self._scene_key, rays_c)
+        ray_grad = torch.empty_like(rays_c) if return_ray_grad else None
+        opts = self._opts(self._scene_key, rays_c, _lib.FLAG_SCRUB_NONFINITE if scrub_nonfinite else 0)
         opts.flags |= self._tape_flag(rays_c, start_c, opts.scene_version)
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream(dev).cuda_stream
-            _lib.check(self._lib.rfb_trace_backward_accumulate(
+            _lib.check(self._lib.rfb_trace_backward_accumulate_rays(
                 self._handle, ctypes.byref(settings), num_points, _ptr(points_c), _ptr(attributes_c),
                 adj_c.numel(), _ptr(adj_c), _ptr(off_c), num_rays, _ptr(rays_c), _ptr(start_c),
                 num_q, _ptr(dq_c), _ptr(di_c), _ptr(rgb_c), _ptr(grad_c), _ptr(dg_c), _ptr(err_c),
-                _ptr(point_error), ctypes.byref(opts), stream))
-        return self.grad_accumulator(dev), point_error
+                _ptr(point_error), _ptr(ray_grad), ctypes.byref(opts), stream))
+        if not return_ray_grad:
+            return self.grad_accumulator(dev), point_error
+        return self.grad_accumulator(dev), point_error, self._caller_order(ray_grad, rays_c, rays_in)
 
     def grad_accumulator(self, device):
         ptr = ctypes.c_void_p()
@@ -536,13 +561,16 @@ class Pipeline:
 
     def trace_backward_params(self, points, point_adjacency, point_adjacency_offsets, rays, start_point, rgb_out,
                               grad_in, depth_quantiles=None, depth_indices=None, depth_grad_in=None, ray_error=None,
-                              weight_threshold=None, max_intersections=None, scrub_nonfinite=True):
-        """Backward of a bound parameter-form scene: gradients of points, att_dc, att_sh and the raw density."""
+                              weight_threshold=None, max_intersections=None, scrub_nonfinite=True,
+                              return_ray_grad=False):
+        """Backward of a bound parameter-form scene: gradients of points, att_dc, att_sh and the raw density,
+        and with ``return_ray_grad`` also ``ray_grad`` (see ``trace_backward``)."""
         if self._params is None:
             raise RuntimeError("no parameter-form scene is bound (bind_scene_params)")
-        _, point_error = self.trace_backward_accumulate(
+        _, point_error, *ray_grad = self.trace_backward_accumulate(
             points, None, point_adjacency, point_adjacency_offsets, rays, start_point, rgb_out, grad_in,
-            depth_quantiles, depth_indices, depth_grad_in, ray_error, weight_threshold, max_intersections)
+            depth_quantiles, depth_indices, depth_grad_in, ray_error, weight_threshold, max_intersections,
+            return_ray_grad=return_ray_grad, scrub_nonfinite=scrub_nonfinite)
         n, dev = points.shape[0], rays.device
         out = {"points_grad": torch.empty((n, 3), dtype=torch.float32, device=dev),
                "att_dc_grad": torch.empty((n, 3), dtype=torch.float32, device=dev),
@@ -556,6 +584,8 @@ class Pipeline:
                 _lib.FLAG_SCRUB_NONFINITE if scrub_nonfinite else 0, stream))
         if point_error is not None:
             out["point_error"] = point_error
+        if return_ray_grad:
+            out["ray_grad"] = ray_grad[0]
         return out
 
     def _scene_tensors(self, points, attributes, point_adjacency, point_adjacency_offsets):

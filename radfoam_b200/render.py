@@ -3,8 +3,9 @@
 Call contract = ``radfoam_model/render.py::TraceRays`` (lines 10-122): nine positional
 arguments ``(pipeline, points, attributes, point_adjacency, point_adjacency_offsets, rays,
 start_point, depth_quantiles, return_contribution)`` in, the 5-tuple ``(rgba, depth,
-contribution, num_intersections, errbox)`` out, gradients for ``points`` and ``attributes``
-only, and ``errbox.ray_error`` (set by the caller between forward and backward) -> ``errbox.point_error``
+contribution, num_intersections, errbox)`` out, gradients for ``points`` and ``attributes`` (and, an
+extension, for ``rays`` when they require grad: ``Pipeline.trace_backward(return_ray_grad=True)``), and
+``errbox.ray_error`` (set by the caller between forward and backward) -> ``errbox.point_error``
 (scene.py:497-548 uses that side channel for the densification error map).  The reference's own file
 runs unmodified on a ``Pipeline`` too (tests/test_gpu_reference_op.py); this op is the native
 counterpart, written for this library:
@@ -69,12 +70,14 @@ class TraceRays(torch.autograd.Function):
         if ctx.with_depth and grad_depth is None:  # depth was returned but not used by the loss
             grad_depth = torch.zeros_like(quantiles)
         box = ctx.errbox
+        want_rays = ctx.needs_input_grad[5]
         grads = ctx.pipeline.trace_backward(points, attributes, adjacency, offsets, rays, start_point, rgba,
                                             grad_rgba, quantiles, depth_indices, grad_depth, box.ray_error,
-                                            scrub_nonfinite=True)
+                                            scrub_nonfinite=True, return_ray_grad=want_rays)
         box.point_error = grads.get("point_error")
         ctx.pipeline = None
-        return (None, grads["points_grad"], grads["attr_grad"]) + (None,) * 6
+        return ((None, grads["points_grad"], grads["attr_grad"], None, None,
+                 grads["ray_grad"] if want_rays else None) + (None,) * 3)
 
 
 class TraceRaysParams(torch.autograd.Function):
@@ -118,13 +121,15 @@ class TraceRaysParams(torch.autograd.Function):
         points, att_dc, att_sh, density, adjacency, offsets, rays, start_point, rgba = saved[:9]
         quantiles, depth_indices = (saved[9], saved[10]) if ctx.with_depth else (None, None)
         pipeline, box = ctx.pipeline, ctx.errbox
+        want_rays = ctx.needs_input_grad[8]
         pipeline.bind_scene_params(att_dc, att_sh, density, ctx.activation_scale)
         try:
             grads = pipeline.trace_backward_params(points, adjacency, offsets, rays, start_point, rgba, grad_rgba,
                                                    quantiles, depth_indices, grad_depth, box.ray_error,
-                                                   scrub_nonfinite=True)
+                                                   scrub_nonfinite=True, return_ray_grad=want_rays)
         finally:
             pipeline.bind_scene_params(None, None, None)
         box.point_error = grads.get("point_error")
         ctx.pipeline = None
-        return (None, grads["points_grad"], grads["att_dc_grad"], grads["att_sh_grad"], grads["density_grad"]) + (None,) * 7
+        return ((None, grads["points_grad"], grads["att_dc_grad"], grads["att_sh_grad"], grads["density_grad"])
+                + (None,) * 3 + (grads.get("ray_grad"),) + (None,) * 3)

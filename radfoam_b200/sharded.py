@@ -242,6 +242,7 @@ class ShardedTracer:
         points_grad, attr_grad = self.reduce_and_finalize(points.shape[0], rays.device, scrub_nonfinite, acc)
         if point_error is not None:
             dist.all_reduce(point_error, op=dist.ReduceOp.SUM, group=self.group)
+        # ray gradients are not computed by the sharded path: ray_grad stays unwritten, as in the reference
         out = {"points_grad": points_grad, "attr_grad": attr_grad, "ray_grad": torch.empty_like(rays)}
         if point_error is not None:
             out["point_error"] = point_error
@@ -251,7 +252,8 @@ class ShardedTracer:
 class ShardedTraceRays(torch.autograd.Function):
     """The render op (radfoam_b200/render.py) over a ShardedTracer: forward on the local ray shard,
     backward yields the all-reduced scene gradients on every rank.  Returns
-    ``(rgba, depth, contribution, num_intersections)`` of the local shard."""
+    ``(rgba, depth, contribution, num_intersections)`` of the local shard.  Unlike ``TraceRays`` it does not
+    compute ray gradients: the gradient for ``rays`` is always ``None``."""
 
     @classmethod
     def apply(cls, tracer, *args):
