@@ -67,6 +67,34 @@ __device__ __forceinline__ void red_add_v4(float *addr, float a, float b, float 
 #endif
 }
 
+// Bulk reduction (sm_90): the TMA unit reads `bytes` (a multiple of 16, both addresses 16-byte aligned) of shared
+// memory at `src` and adds them as f32 into global memory at `dst`, so the LSU issues no request per 16 bytes and
+// L2 receives whole sectors.  Each call is its own bulk group of the calling thread.  Shared-memory writes to `src`
+// must be made visible to the async proxy first (fence_proxy_async_smem), and `src` may be rewritten only after
+// bulk_wait_read.
+__device__ __forceinline__ void bulk_red_add_f32(float *dst, const float *src, uint32_t bytes) {
+#ifdef RFB_EMU // element by element with the emulator's atomics, done at issue (the hardware's order is unspecified)
+    for (uint32_t i = 0; i < bytes / 4; ++i)
+        atomicAdd(dst + i, src[i]);
+#else
+    asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;\n\t"
+                 "cp.async.bulk.commit_group;" ::"l"(dst),
+                 "r"(static_cast<uint32_t>(__cvta_generic_to_shared(src))), "r"(bytes)
+                 : "memory");
+#endif
+}
+__device__ __forceinline__ void fence_proxy_async_smem() {
+#ifndef RFB_EMU
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+#endif
+}
+// waits until every bulk operation this thread issued has finished reading its shared-memory source
+__device__ __forceinline__ void bulk_wait_read() {
+#ifndef RFB_EMU
+    asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+#endif
+}
+
 // NVSwitch multicast (NVLS): one load returns the SUM of the word at the same offset of every GPU's copy -- the
 // switch does the reduction --, one store writes all copies.  `p` is an address in the multicast mapping of a
 // symmetric allocation.

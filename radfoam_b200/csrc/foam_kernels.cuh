@@ -783,18 +783,21 @@ __global__ void __launch_bounds__(kBlock) backward_kernel(const BackwardParams p
 // sliver cell the other misses and they drift out of lock-step), so instead of 13 x 128-bit
 // reductions per lane per step the warp keeps a small direct-mapped cache of gradient rows in
 // shared memory:
-//   * lanes are grouped by cell (MATCH.ANY); a lane that is alone in its cell issues its
-//     reductions directly, in parallel with the other singleton lanes;
-//   * every lane of a multi-lane group writes its row (SH products + density grad) to a
-//     staging row in shared memory; the warp sums the staged rows of a group "transposed" --
+//   * every lane with a row this step writes it (SH products + density grad) to its own
+//     staging row in shared memory;
+//   * lanes are grouped by cell (MATCH.ANY); a lane in a group of fewer than MIN_GROUP lanes
+//     sends its staged row to HBM as one bulk reduction (cp.reduce.async.bulk: the TMA unit reads
+//     the row, so the LSU issues no request per 16 bytes), and waits for that read to finish only
+//     when it next rewrites the row, a step later;
+//   * the warp sums the staged rows of a larger group "transposed" --
 //     lane j owns elements 2j, 2j+1 of the row -- so the shared-memory update needs no atomics
 //     and has no bank conflicts, and adds the sum to the cell's cache row;
 //   * a cache row is written to HBM (13 lanes x one RED.128) only when its slot is claimed by
 //     another cell, or when the warp's rays are finished.
 // Position gradients (3 floats to the previous composited cell) stay direct reductions.
-// MIN_GROUP: smallest same-cell lane group routed through the cache (smaller groups reduce
-// directly: all such lanes issue their 13 reductions simultaneously, which costs fewer issue
-// slots than one serial cache round per group, at the price of more L2 atomic traffic).
+// MIN_GROUP: smallest same-cell lane group routed through the cache (smaller groups send one
+// bulk reduction per lane, which costs fewer issue slots than one serial cache round per group,
+// at the price of more L2 atomic traffic).
 // REPLAY = true: the steps come from the forward's tape of (cell, t1) instead of re-scanning
 // faces.  When a tape is offered the host launches both instantiations back to back; each looks
 // at the tape's overflow flag first and exactly one of them does the work (the other returns at
@@ -815,6 +818,7 @@ __global__ void __launch_bounds__(kBlock, MIN_BLOCKS * 128 / kBlock)
     constexpr unsigned FULL = 0xffffffffu;
     static_assert(HALF_ROW <= 32, "row too wide for one warp pass");
     static_assert((SLOTS & (SLOTS - 1)) == 0, "SLOTS must be a power of two");
+    static_assert(GR % 4 == 0 && SR % 4 == 0, "stage rows and bulk reductions need 16-byte multiples");
 
 #ifdef RFB_EMU
     float *smem = rfb_emu_dynamic_smem();
@@ -960,22 +964,28 @@ __global__ void __launch_bounds__(kBlock, MIN_BLOCKS * 128 / kBlock)
         unsigned grp = __match_any_sync(FULL, c_valid ? c_cell : (0x80000000u | lane));
         bool single = c_valid && __popc(grp) < MIN_GROUP;
         bool staged = c_valid && !single;
-        if (single)
-            reduce_row_direct<DEG>(p.acc + (uint64_t)c_cell * GR, sh, dL_drgb, dL_ds);
+        if (c_valid) {
+            bulk_wait_read(); // this lane's previous bulk reduction has finished reading its stage row
+            float4 *srow = reinterpret_cast<float4 *>(stage + lane * GR);
+#pragma unroll
+            for (int i = 0; i < SR; i += 4) {
+                float v[4];
+#pragma unroll
+                for (int k = 0; k < 4; ++k)
+                    v[k] = (i + k < 3 * sh_dim(DEG)) ? __fmul_rn(sh[(i + k) / 3], dL_drgb[(i + k) % 3]) : 0.0f;
+                srow[i / 4] = make_float4(v[0], v[1], v[2], v[3]);
+            }
+            srow[SR / 4] = make_float4(dL_ds, 0.0f, 0.0f, 0.0f);
+        }
+        if (single) {
+            // the whole row as one bulk reduction; a row whose three channel gradients are all zero sends
+            // its density slot only
+            const uint32_t off = (dL_drgb[0] != 0.0f || dL_drgb[1] != 0.0f || dL_drgb[2] != 0.0f) ? 0 : SR;
+            fence_proxy_async_smem();
+            bulk_red_add_f32(p.acc + (uint64_t)c_cell * GR + off, stage + lane * GR + off, (GR - off) * 4);
+        }
         unsigned todo = __ballot_sync(FULL, staged);
         if (todo) {
-            if (staged) {
-                float4 *srow = reinterpret_cast<float4 *>(stage + lane * GR);
-#pragma unroll
-                for (int i = 0; i < SR; i += 4) {
-                    float v[4];
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        v[k] = (i + k < 3 * sh_dim(DEG)) ? __fmul_rn(sh[(i + k) / 3], dL_drgb[(i + k) % 3]) : 0.0f;
-                    srow[i / 4] = make_float4(v[0], v[1], v[2], v[3]);
-                }
-                srow[SR / 4] = make_float4(dL_ds, 0.0f, 0.0f, 0.0f);
-            }
             __syncwarp();
             while (todo) {
                 int leader = __ffs(todo) - 1;
@@ -1043,6 +1053,7 @@ __global__ void __launch_bounds__(kBlock, MIN_BLOCKS * 128 / kBlock)
             red_add_v4(p.acc + (uint64_t)tag * GR + 4 * lane, v.x, v.y, v.z, v.w);
         }
     }
+    bulk_wait_read(); // shared memory must outlive the bulk reductions' reads
     if (RAY && has_ray)
         ray_grad_store<DEG>(p, rg, r, ray, ra, G);
 }
