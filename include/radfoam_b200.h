@@ -11,6 +11,7 @@
  *   rfb_trace_forward        <- Pipeline::trace_forward             src/tracing/pipeline.h:62-78
  *   rfb_trace_backward       <- Pipeline::trace_backward            src/tracing/pipeline.h:80-100
  *   rfb_trace_benchmark      <- Pipeline::trace_benchmark           src/tracing/pipeline.h:117-126
+ *   rfb_trace_visualization <- Pipeline::trace_visualization src/tracing/pipeline.h:102-115
  *
  * The reference interface is a C++ vtable taking raw device pointers (Eigen
  * types appear only as reinterpret_casts of packed floats); this header
@@ -300,6 +301,59 @@ int rfb_trace_benchmark(rfb_pipeline *pipeline, const rfb_trace_settings *settin
                         const void *adjacent_diff, const rfb_camera *camera,
                         const uint32_t *start_point_index, uint32_t *output_rgba,
                         const rfb_launch_opts *opts, void *stream);
+
+/* radfoam::VisualizationMode, src/tracing/pipeline.h:22-27 */
+enum { RFB_VIS_RGB = 0, RFB_VIS_DEPTH = 1, RFB_VIS_ALPHA = 2, RFB_VIS_INTERSECTIONS = 3 };
+
+/* radfoam::ColorMap, src/utils/typing.h:136-141 (an index into rfb_cmap_table) */
+enum { RFB_CMAP_GRAY = 0, RFB_CMAP_VIRIDIS = 1, RFB_CMAP_INFERNO = 2, RFB_CMAP_TURBO = 3 };
+
+/* radfoam::VisualizationSettings, src/tracing/pipeline.h:29-47 (defaults: RGB, Turbo,
+ * bg (1, 1, 1), no checker, max_depth 10, depth_quantile 0.5) */
+typedef struct rfb_visualization_settings {
+    int32_t mode;      /* RFB_VIS_* */
+    int32_t color_map; /* RFB_CMAP_*: the table used by the depth and intersections modes */
+    float bg_color[3]; /* RGB mode: background seen through the remaining transmittance */
+    uint32_t checker_bg; /* nonzero: a 20-pixel 0.3 / 0.5 grey checker instead of bg_color */
+    float max_depth;      /* depth mode: the depth mapped to the end of the colour map */
+    float depth_quantile; /* depth mode: the depth where transmittance first drops below this */
+} rfb_visualization_settings;
+
+/* radfoam::CMapTable, src/utils/typing.h:143-146.  Both arrays are DEVICE memory owned by the caller:
+ * data[m] points at sizes[m] >= 1 RGB entries (float[sizes[m]][3]) of colour map m, for m in RFB_CMAP_*.
+ * The library ships no colour-map data. */
+typedef struct rfb_cmap_table {
+    const float *const *data;
+    const int32_t *sizes;
+} rfb_cmap_table;
+
+/* Preview render with in-kernel ray generation, as rfb_trace_benchmark, but with the settings' output
+ * (RFB_VIS_RGB: colour over a background; RFB_VIS_DEPTH: colormap(depth / max_depth); RFB_VIS_ALPHA: 1 - T;
+ * RFB_VIS_INTERSECTIONS: colormap((cells entered - 1) / max_intersections)) written as RGBA8 words to a 2-D
+ * surface: pixel (i, j) goes to byte column 4 i of row height - 1 - j (bottom-up, for GL).  output_surface is a
+ * cudaSurfaceObject_t of at least width x height 4-byte texels.  start_index is the entry cell, by value;
+ * num_tets is accepted and ignored, as in the reference.  cmap_table may be NULL for the RGB and alpha modes. */
+int rfb_trace_visualization(rfb_pipeline *pipeline, const rfb_trace_settings *settings,
+                            const rfb_visualization_settings *vis_settings,
+                            const rfb_camera *camera, const rfb_cmap_table *cmap_table,
+                            uint32_t num_points, uint32_t num_tets, const float *points,
+                            const void *attributes, const uint32_t *point_adjacency,
+                            const uint32_t *point_adjacency_offsets,
+                            const void *adjacent_diff, uint32_t start_index,
+                            uint64_t output_surface, const rfb_launch_opts *opts,
+                            void *stream);
+
+/* rfb_trace_visualization into a linear buffer: output_rgba is u32[height][width] in the surface's row order
+ * (the frame equals a 2-D copy of the surface rfb_trace_visualization would fill). */
+int rfb_trace_visualization_rgba8(rfb_pipeline *pipeline, const rfb_trace_settings *settings,
+                                  const rfb_visualization_settings *vis_settings,
+                                  const rfb_camera *camera, const rfb_cmap_table *cmap_table,
+                                  uint32_t num_points, uint32_t num_tets, const float *points,
+                                  const void *attributes, const uint32_t *point_adjacency,
+                                  const uint32_t *point_adjacency_offsets,
+                                  const void *adjacent_diff, uint32_t start_index,
+                                  uint32_t *output_rgba, const rfb_launch_opts *opts,
+                                  void *stream);
 
 /* kernels launched by this library (all threads of the process) since the last reset
  * (bench.py reports it as gpu_launches) */

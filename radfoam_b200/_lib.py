@@ -40,6 +40,18 @@ class LaunchOpts(ctypes.Structure):  # rfb_launch_opts
     _fields_ = [("scene_version", c_uint64), ("image_width", c_uint32), ("flags", c_uint32)]
 
 
+class VisualizationSettings(ctypes.Structure):  # rfb_visualization_settings
+    _fields_ = [("mode", c_int32), ("color_map", c_int32), ("bg_color", c_float * 3), ("checker_bg", c_uint32),
+                ("max_depth", c_float), ("depth_quantile", c_float)]
+
+
+class CMapTable(ctypes.Structure):  # rfb_cmap_table (two device pointers)
+    _fields_ = [("data", c_void_p), ("sizes", c_void_p)]
+
+
+VIS_MODES = {"rgb": 0, "depth": 1, "alpha": 2, "intersections": 3}  # RFB_VIS_*
+COLOR_MAPS = {"gray": 0, "viridis": 1, "inferno": 2, "turbo": 3}  # RFB_CMAP_*
+
 FLAG_SCRUB_NONFINITE = 1
 FLAG_RECORD_TAPE = 2
 FLAG_USE_TAPE = 4
@@ -80,6 +92,12 @@ SIGNATURES = {
                                           POINTER(Multicast), c_uint32, _P]),
     "rfb_trace_benchmark": (c_int, [_P, POINTER(TraceSettings), c_uint32, _P, _P, _P, _P, _P,
                                     POINTER(Camera), _P, _P, POINTER(LaunchOpts), _P]),
+    "rfb_trace_visualization": (c_int, [_P, POINTER(TraceSettings), POINTER(VisualizationSettings),
+                                        POINTER(Camera), POINTER(CMapTable), c_uint32, c_uint32, _P, _P, _P, _P,
+                                        _P, c_uint32, c_uint64, POINTER(LaunchOpts), _P]),
+    "rfb_trace_visualization_rgba8": (c_int, [_P, POINTER(TraceSettings), POINTER(VisualizationSettings),
+                                              POINTER(Camera), POINTER(CMapTable), c_uint32, c_uint32, _P, _P, _P,
+                                              _P, _P, c_uint32, _P, POINTER(LaunchOpts), _P]),
     "rfb_launch_count": (c_uint64, []),
     "rfb_reset_launch_count": (None, []),
     "rfb_device_alloc_counts": (None, [POINTER(c_uint64), POINTER(c_uint64)]),

@@ -1555,4 +1555,173 @@ __global__ void __launch_bounds__(kBlock) benchmark_kernel(const BenchmarkParams
     p.out[r] = pack_rgba8(cr, cg, cb, 1.0f);
 }
 
+// ------------------------------------------------------------------ visualization
+// Pipeline::trace_visualization (pipeline.h:102-115, kernel pipeline.cu:345-470): the benchmark frame's walk
+// plus a quantile depth and the step count, and one of four outputs chosen by a uniform runtime branch.
+enum VisMode { kVisRGB = 0, kVisDepth = 1, kVisAlpha = 2, kVisIntersections = 3 };
+
+// CMapTable (typing.h:143-146): caller-owned device tables, indexed by colour map; data[m] is float[sizes[m]][3]
+struct CMapTable {
+    const float *const *data;
+    const int *sizes;
+};
+
+struct VisualizationParams {
+    const float4 *cells;
+    const float *sh_rows;
+    CameraParams cam;
+    uint32_t start;
+    uint32_t blocks_x;
+    float weight_threshold;
+    uint32_t max_steps;
+    int mode;
+    int color_map;
+    float bg[3];
+    uint32_t checker_bg;
+    float max_depth;
+    float depth_quantile;
+    CMapTable cmap;
+    uint32_t *exact_flag;
+};
+
+// The frame goes to a surface (what the reference writes: surf2Dwrite at byte column 4x, trap on out-of-range) or
+// to a linear uint32[height][width] buffer; both in the surface's bottom-up row order.
+#ifdef RFB_EMU
+// The CPU kernel-logic emulator has no surfaces: there the handle is the address of an RfbEmuSurface, and a store
+// outside it aborts where the device's default boundary mode traps.
+struct RfbEmuSurface {
+    void *data;
+    uint64_t pitch; // bytes per row
+    uint32_t width_bytes, height;
+};
+#endif
+struct SurfaceOut {
+    cudaSurfaceObject_t surf;
+    __device__ __forceinline__ void store(uint32_t x, uint32_t y, uint32_t v) const {
+#ifdef RFB_EMU
+        const RfbEmuSurface *s = reinterpret_cast<const RfbEmuSurface *>(surf);
+        if ((uint64_t)4u * x + 4u > s->width_bytes || y >= s->height)
+            abort();
+        memcpy(static_cast<char *>(s->data) + (uint64_t)y * s->pitch + 4u * (uint64_t)x, &v, 4);
+#else
+        surf2Dwrite(v, surf, (int)(4u * x), (int)y);
+#endif
+    }
+};
+struct LinearOut {
+    uint32_t *out;
+    uint32_t width;
+    __device__ __forceinline__ void store(uint32_t x, uint32_t y, uint32_t v) const {
+        out[(uint64_t)y * width + x] = v;
+    }
+};
+
+// cvt.rzi.s32.f32, with its rules for NaN (-> 0) and out-of-range values (saturation at INT_MIN / INT_MAX) written
+// out, so that the same source means the same thing where a plain cast would be undefined (the CPU emulator).
+__device__ __forceinline__ int f2i_rz_sat(float x) {
+    if (x != x)
+        return 0;
+    if (x >= 2147483648.0f)
+        return 2147483647;
+    if (x < -2147483648.0f)
+        return (int)0x80000000u;
+    return (int)x;
+}
+
+// The .SAT modifier: clamp to [+0, 1], NaN -> +0.
+__device__ __forceinline__ float sat_unit(float x) { return x > 0.0f ? (x < 1.0f ? x : 1.0f) : 0.0f; }
+
+// The reference's clamps fold into the .SAT of the instruction that makes the value (FFMA.SAT / FADD.SAT in its
+// SASS, visualization<float,0,128>), so a NaN channel becomes 0, not the 255 std::min/std::max would give.
+// r, g, b are already in [0, 1].
+__device__ __forceinline__ uint32_t pack_unit_rgb8(float r, float g, float b) {
+    const uint32_t ri = (uint32_t)(int)__fmul_rn(r, 255.0f);
+    const uint32_t gi = (uint32_t)(int)__fmul_rn(g, 255.0f);
+    const uint32_t bi = (uint32_t)(int)__fmul_rn(b, 255.0f);
+    return 0xff000000u | (bi << 16) | (gi << 8) | ri;
+}
+
+// colormap (tracing_utils.cuh:117-130), association read from the reference's SASS (visualization<float,0,128>):
+//   p = (float)(L - 1) * v;  i0 = cvt.rzi.s32(p)  (NaN -> 0, saturating at INT_MIN / INT_MAX);  t = p - (float)i0
+//   i1 = i0 + 1 (32-bit wrap);  both clamped to [0, L - 1]
+//   c_k = sat(fma(1 - t, table[i0]_k, t * table[i1]_k))
+__device__ __forceinline__ uint32_t colormap_rgba8(float v, int map, const CMapTable &cm) {
+    const int last = cm.sizes[map] - 1;
+    const float *vals = cm.data[map];
+    const float pos = __fmul_rn((float)last, v);
+    const int i0 = f2i_rz_sat(pos);
+    const int i1 = (int)((uint32_t)i0 + 1u);
+    const float t = __fsub_rn(pos, (float)i0);
+    const float u = __fsub_rn(1.0f, t);
+    const float *a = vals + 3 * (int64_t)max(0, min(i0, last));
+    const float *b = vals + 3 * (int64_t)max(0, min(i1, last));
+    return pack_unit_rgb8(sat_unit(__fmaf_rn(u, a[0], __fmul_rn(t, b[0]))),
+                          sat_unit(__fmaf_rn(u, a[1], __fmul_rn(t, b[1]))),
+                          sat_unit(__fmaf_rn(u, a[2], __fmul_rn(t, b[2]))));
+}
+
+template <int DEG, typename Faces, int MODE, typename Out>
+__global__ void __launch_bounds__(kBlock) visualization_kernel(const VisualizationParams p, const Faces fa,
+                                                               const Out out) {
+    if (MODE == kScanExactTwin && *p.exact_flag == 0u)
+        return;
+    uint32_t r;
+    if (!thread_ray(p.cam.width * p.cam.height, p.cam.width, p.blocks_x, r))
+        return;
+    const uint32_t pi = r % p.cam.width, pj = r / p.cam.width;
+    const uint32_t row = p.cam.height - 1u - pj;
+    RayGeom ray;
+    cast_ray(p.cam, (int)pi, (int)pj, ray);
+    float nrm = __fsqrt_rn(__fmaf_rn(ray.dx, ray.dx, __fmaf_rn(ray.dy, ray.dy, __fmul_rn(ray.dz, ray.dz))));
+    if (nrm < 0.1f) {
+        out.store(pi, row, 0u);
+        return;
+    }
+    float sh[sh_dim(DEG)];
+    sh_basis<DEG>(ray.dx, ray.dy, ray.dz, sh);
+    const float q = p.depth_quantile;
+    float T = 1.0f, cr = 0.0f, cg = 0.0f, cb = 0.0f;
+    float depth = 0.0f;
+    bool passed = false;
+    auto cell_fn = [&](uint32_t cell, const float4 &pc, float t0, float t1, const float4 &) -> bool {
+        float s = pc.w;
+        float r_ = 0.0f, g_ = 0.0f, b_ = 0.0f;
+        if (s > 1e-6f)
+            sh_to_rgb<DEG>(p.sh_rows + (uint64_t)cell * sh_row(DEG), sh, r_, g_, b_);
+        float delta = fmaxf(__fsub_rn(t1, t0), 0.0f);
+        float alpha = 1.0f - expf(-s * delta);
+        float w = __fmul_rn(T, alpha);
+        cr = __fmaf_rn(w, r_, cr);
+        cg = __fmaf_rn(w, g_, cg);
+        cb = __fmaf_rn(w, b_, cb);
+        float Tn = __fmul_rn(T, __fsub_rn(1.0f, alpha));
+        if (!passed && Tn < q) { // the forward's quantile depth, first quantile only
+            depth = __fadd_rn(t0, __fdiv_rn(logf(__fdiv_rn(T, q)), s));
+            passed = true;
+        }
+        T = Tn;
+        return T > p.weight_threshold;
+    };
+    if (MODE == kScanFast && needs_exact_scan(ray.dx, ray.dy, ray.dz))
+        *p.exact_flag = 1u;
+    const uint32_t n = walk<MODE == kScanExactTwin>(fa, p.cells, ray, p.start, p.max_steps, cell_fn);
+
+    uint32_t v;
+    if (p.mode == kVisRGB) {
+        float bg0 = p.bg[0], bg1 = p.bg[1], bg2 = p.bg[2];
+        if (p.checker_bg) // 20-pixel checker: 0.3 where the two square parities agree, else 0.5
+            bg0 = bg1 = bg2 = (((pi / 20u) ^ (pj / 20u)) & 1u) ? 0.5f : 0.3f;
+        v = pack_unit_rgb8(sat_unit(__fmaf_rn(T, bg0, cr)), sat_unit(__fmaf_rn(T, bg1, cg)),
+                           sat_unit(__fmaf_rn(T, bg2, cb)));
+    } else if (p.mode == kVisDepth) {
+        v = colormap_rgba8(__fdiv_rn(depth, p.max_depth), p.color_map, p.cmap);
+    } else if (p.mode == kVisAlpha) {
+        const float a = sat_unit(__fsub_rn(1.0f, T));
+        v = pack_unit_rgb8(a, a, a);
+    } else {
+        v = colormap_rgba8(__fdiv_rn(__uint2float_rn(n - 1u), __uint2float_rn(p.max_steps)), p.color_map, p.cmap);
+    }
+    out.store(pi, row, v);
+}
+
 } // namespace rfb

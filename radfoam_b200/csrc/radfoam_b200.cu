@@ -551,11 +551,132 @@ int launch_benchmark(int deg, const BenchmarkParams &bp, const Faces &fa, uint32
     return launch_benchmark_mode<Faces, kScanExactTwin>(deg, bp, fa, blocks, stream);
 }
 
+template <typename Faces, int MODE, typename Out>
+int launch_visualization_mode(int deg, const VisualizationParams &vp, const Faces &fa, const Out &out,
+                              uint32_t blocks, cudaStream_t stream) {
+    switch (deg) {
+    case 0: RFB_LAUNCH((visualization_kernel<0, Faces, MODE, Out>), blocks, kBlock, 0, stream, vp, fa, out); break;
+    case 1: RFB_LAUNCH((visualization_kernel<1, Faces, MODE, Out>), blocks, kBlock, 0, stream, vp, fa, out); break;
+    case 2: RFB_LAUNCH((visualization_kernel<2, Faces, MODE, Out>), blocks, kBlock, 0, stream, vp, fa, out); break;
+    default: RFB_LAUNCH((visualization_kernel<3, Faces, MODE, Out>), blocks, kBlock, 0, stream, vp, fa, out); break;
+    }
+    RFB_LAUNCHED();
+    return 0;
+}
+
+template <typename Faces, typename Out>
+int launch_visualization(int deg, const VisualizationParams &vp, const Faces &fa, const Out &out, uint32_t blocks,
+                         cudaStream_t stream) {
+    if (int rc = launch_visualization_mode<Faces, kScanFast>(deg, vp, fa, out, blocks, stream))
+        return rc;
+    return launch_visualization_mode<Faces, kScanExactTwin>(deg, vp, fa, out, blocks, stream);
+}
+
 rfb_trace_settings settings_or_default(const rfb_trace_settings *s) {
     rfb_trace_settings d;
     d.weight_threshold = 0.001f; // default_trace_settings(), pipeline.h:15-20
     d.max_intersections = 1024;
     return s ? *s : d;
+}
+
+CameraParams camera_params(const rfb_camera *camera) {
+    CameraParams c;
+    memcpy(c.position, camera->position, sizeof(float) * 3);
+    memcpy(c.forward, camera->forward, sizeof(float) * 3);
+    memcpy(c.right, camera->right, sizeof(float) * 3);
+    memcpy(c.up, camera->up, sizeof(float) * 3);
+    c.fov = camera->fov;
+    c.width = camera->width;
+    c.height = camera->height;
+    c.model = camera->model;
+    return c;
+}
+
+// Scene mirrors for the entry points that take the caller's half4 adjacent_diff (trace_benchmark,
+// trace_visualization).  The reference interface does not pass the adjacency size (pipeline.h:102-126); it is
+// offsets[N].  Reading it costs a stream sync, paid only when the mirrors are (re)built.
+int ensure_diff_scene(rfb_pipeline *p, uint32_t num_points, const float *points, const void *attributes,
+                      const uint32_t *point_adjacency, const uint32_t *point_adjacency_offsets,
+                      const void *adjacent_diff, const rfb_launch_opts *opts, cudaStream_t stream) {
+    uint32_t num_edges = p->key_valid ? p->key.e : 0;
+    {
+        SceneKey probe;
+        probe.points = points;
+        probe.attrs = attributes;
+        probe.adj = point_adjacency;
+        probe.off = point_adjacency_offsets;
+        probe.diff = adjacent_diff;
+        probe.n = num_points;
+        probe.e = num_edges;
+        probe.version = opts ? opts->scene_version : 0;
+        bool hit = p->key_valid && probe.version != 0 && probe == p->key && p->key.faces;
+        if (!hit) {
+            RFB_CUDA(cudaMemcpyAsync(&num_edges, point_adjacency_offsets + num_points, sizeof(uint32_t),
+                                     cudaMemcpyDeviceToHost, stream));
+            RFB_CUDA(cudaStreamSynchronize(stream));
+        }
+    }
+    return ensure_scene(p, num_points, points, attributes, num_edges, point_adjacency, point_adjacency_offsets,
+                        true, opts, stream, adjacent_diff);
+}
+
+// Shared body of rfb_trace_visualization{,_rgba8}: checks, mirrors, parameters, launch into `out`.
+template <typename Out>
+int trace_visualization(const char *fn, rfb_pipeline *p, const rfb_trace_settings *settings,
+                        const rfb_visualization_settings *vis, const rfb_camera *camera,
+                        const rfb_cmap_table *cmap_table, uint32_t num_points, const float *points,
+                        const void *attributes, const uint32_t *point_adjacency,
+                        const uint32_t *point_adjacency_offsets, const void *adjacent_diff, uint32_t start_index,
+                        bool have_output, Out out, const rfb_launch_opts *opts, void *stream_) {
+    const std::string name(fn);
+    if (!p)
+        return fail(name + ": pipeline is NULL");
+    if (!vis || !camera || !points || !attributes || !point_adjacency || !point_adjacency_offsets ||
+        !adjacent_diff || !have_output)
+        return fail(name + ": NULL argument");
+    if (vis->mode < RFB_VIS_RGB || vis->mode > RFB_VIS_INTERSECTIONS)
+        return fail(name + ": unknown visualization mode " + std::to_string(vis->mode));
+    if (vis->color_map < RFB_CMAP_GRAY || vis->color_map > RFB_CMAP_TURBO)
+        return fail(name + ": unknown color map " + std::to_string(vis->color_map));
+    const bool uses_cmap = vis->mode == RFB_VIS_DEPTH || vis->mode == RFB_VIS_INTERSECTIONS;
+    if (uses_cmap && (!cmap_table || !cmap_table->data || !cmap_table->sizes))
+        return fail(name + ": the depth and intersections modes need a color map table");
+    if (camera->model != RFB_PINHOLE && camera->model != RFB_FISHEYE)
+        return fail("Invalid camera model");
+    if (start_index >= num_points)
+        return fail(name + ": start_index is not a point of the scene");
+    if (camera->width == 0 || camera->height == 0)
+        return 0;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (int rc = ensure_diff_scene(p, num_points, points, attributes, point_adjacency, point_adjacency_offsets,
+                                   adjacent_diff, opts, stream))
+        return rc;
+    rfb_trace_settings s = settings_or_default(settings);
+    VisualizationParams vp;
+    vp.cells = reinterpret_cast<const float4 *>(p->cells.ptr);
+    vp.sh_rows = reinterpret_cast<const float *>(p->sh_rows.ptr);
+    vp.cam = camera_params(camera);
+    vp.start = start_index;
+    vp.weight_threshold = s.weight_threshold;
+    vp.max_steps = s.max_intersections;
+    vp.mode = vis->mode;
+    vp.color_map = vis->color_map;
+    memcpy(vp.bg, vis->bg_color, sizeof(float) * 3);
+    vp.checker_bg = vis->checker_bg;
+    vp.max_depth = vis->max_depth;
+    vp.depth_quantile = vis->depth_quantile;
+    vp.cmap.data = uses_cmap ? cmap_table->data : nullptr;
+    vp.cmap.sizes = uses_cmap ? cmap_table->sizes : nullptr;
+    RFB_CUDA(p->scan_flag.ensure(4 * sizeof(uint32_t)));
+    RFB_CUDA(cudaMemsetAsync(p->scan_flag.ptr, 0, 4 * sizeof(uint32_t), stream));
+    vp.exact_flag = reinterpret_cast<uint32_t *>(p->scan_flag.ptr);
+    vp.blocks_x = (camera->width + kTileW - 1) / kTileW;
+    uint32_t blocks = vp.blocks_x * ((camera->height + kTileH - 1) / kTileH);
+    PaddedFaces fa;
+    fa.faces = reinterpret_cast<const uint2 *>(p->faces.ptr);
+    fa.nbr = reinterpret_cast<const uint32_t *>(p->nbr.ptr);
+    fa.off = point_adjacency_offsets;
+    return launch_visualization(p->sh_degree, vp, fa, out, blocks, stream);
 }
 
 } // namespace
@@ -1209,28 +1330,8 @@ int rfb_trace_benchmark(rfb_pipeline *p, const rfb_trace_settings *settings, uin
     if (camera->width == 0 || camera->height == 0)
         return 0;
     cudaStream_t stream = (cudaStream_t)stream_;
-    // The reference interface does not pass the adjacency size (pipeline.h:117-126); it is
-    // offsets[N].  Reading it costs a stream sync, paid only when the mirrors are (re)built.
-    uint32_t num_edges = p->key_valid ? p->key.e : 0;
-    {
-        SceneKey probe;
-        probe.points = points;
-        probe.attrs = attributes;
-        probe.adj = point_adjacency;
-        probe.off = point_adjacency_offsets;
-        probe.diff = adjacent_diff;
-        probe.n = num_points;
-        probe.e = num_edges;
-        probe.version = opts ? opts->scene_version : 0;
-        bool hit = p->key_valid && probe.version != 0 && probe == p->key && p->key.faces;
-        if (!hit) {
-            RFB_CUDA(cudaMemcpyAsync(&num_edges, point_adjacency_offsets + num_points, sizeof(uint32_t),
-                                     cudaMemcpyDeviceToHost, stream));
-            RFB_CUDA(cudaStreamSynchronize(stream));
-        }
-    }
-    if (int rc = ensure_scene(p, num_points, points, attributes, num_edges, point_adjacency,
-                              point_adjacency_offsets, true, opts, stream, adjacent_diff))
+    if (int rc = ensure_diff_scene(p, num_points, points, attributes, point_adjacency, point_adjacency_offsets,
+                                   adjacent_diff, opts, stream))
         return rc;
     rfb_trace_settings s = settings_or_default(settings);
     BenchmarkParams bp;
@@ -1238,14 +1339,7 @@ int rfb_trace_benchmark(rfb_pipeline *p, const rfb_trace_settings *settings, uin
     bp.sh_rows = reinterpret_cast<const float *>(p->sh_rows.ptr);
     bp.start = start_point_index;
     bp.out = output_rgba;
-    memcpy(bp.cam.position, camera->position, sizeof(float) * 3);
-    memcpy(bp.cam.forward, camera->forward, sizeof(float) * 3);
-    memcpy(bp.cam.right, camera->right, sizeof(float) * 3);
-    memcpy(bp.cam.up, camera->up, sizeof(float) * 3);
-    bp.cam.fov = camera->fov;
-    bp.cam.width = camera->width;
-    bp.cam.height = camera->height;
-    bp.cam.model = camera->model;
+    bp.cam = camera_params(camera);
     bp.weight_threshold = s.weight_threshold;
     bp.max_steps = s.max_intersections;
     RFB_CUDA(p->scan_flag.ensure(4 * sizeof(uint32_t)));
@@ -1259,6 +1353,37 @@ int rfb_trace_benchmark(rfb_pipeline *p, const rfb_trace_settings *settings, uin
     fa.nbr = reinterpret_cast<const uint32_t *>(p->nbr.ptr);
     fa.off = point_adjacency_offsets;
     return launch_benchmark(p->sh_degree, bp, fa, blocks, stream);
+}
+
+int rfb_trace_visualization(rfb_pipeline *p, const rfb_trace_settings *settings,
+                            const rfb_visualization_settings *vis_settings, const rfb_camera *camera,
+                            const rfb_cmap_table *cmap_table, uint32_t num_points, uint32_t num_tets,
+                            const float *points, const void *attributes, const uint32_t *point_adjacency,
+                            const uint32_t *point_adjacency_offsets, const void *adjacent_diff,
+                            uint32_t start_index, uint64_t output_surface, const rfb_launch_opts *opts,
+                            void *stream) {
+    (void)num_tets; // accepted and unused, as in the reference
+    SurfaceOut out;
+    out.surf = (cudaSurfaceObject_t)output_surface;
+    return trace_visualization("rfb_trace_visualization", p, settings, vis_settings, camera, cmap_table, num_points,
+                               points, attributes, point_adjacency, point_adjacency_offsets, adjacent_diff,
+                               start_index, output_surface != 0, out, opts, stream);
+}
+
+int rfb_trace_visualization_rgba8(rfb_pipeline *p, const rfb_trace_settings *settings,
+                                  const rfb_visualization_settings *vis_settings, const rfb_camera *camera,
+                                  const rfb_cmap_table *cmap_table, uint32_t num_points, uint32_t num_tets,
+                                  const float *points, const void *attributes, const uint32_t *point_adjacency,
+                                  const uint32_t *point_adjacency_offsets, const void *adjacent_diff,
+                                  uint32_t start_index, uint32_t *output_rgba, const rfb_launch_opts *opts,
+                                  void *stream) {
+    (void)num_tets;
+    LinearOut out;
+    out.out = output_rgba;
+    out.width = camera ? camera->width : 0u;
+    return trace_visualization("rfb_trace_visualization_rgba8", p, settings, vis_settings, camera, cmap_table,
+                               num_points, points, attributes, point_adjacency, point_adjacency_offsets,
+                               adjacent_diff, start_index, output_rgba != nullptr, out, opts, stream);
 }
 
 } // extern "C"

@@ -691,6 +691,106 @@ class Pipeline:
                 _ptr(output_rgba), ctypes.byref(opts), stream))
         return None
 
+    @staticmethod
+    def _camera(camera):
+        cam = _lib.Camera()
+        for key in ("position", "forward", "up", "right"):
+            vec = camera[key]
+            vals = [float(v) for v in (vec.detach().cpu().reshape(-1).tolist()
+                                       if isinstance(vec, torch.Tensor) else list(vec))]
+            getattr(cam, key)[:] = vals[:3]
+        cam.fov = float(camera["fov"])
+        cam.width = int(camera["width"])
+        cam.height = int(camera["height"])
+        if camera["model"] not in ("pinhole", "fisheye"):
+            raise RuntimeError("Invalid camera model")
+        cam.model = 0 if camera["model"] == "pinhole" else 1
+        return cam
+
+    def _cmap_arrays(self, cmap_table, device):
+        """Device arrays (pointer table, lengths) of a colour-map table: four float32 CUDA tensors [L_k, 3].
+        Built once per table; the tensors are held so the pointers stay valid."""
+        tables = tuple(cmap_table)
+        if len(tables) != 4:
+            raise RuntimeError("cmap_table must hold one [L, 3] table per colour map (gray, viridis, inferno, turbo)")
+        for t in tables:
+            if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or t.device != device:
+                raise RuntimeError("cmap_table entries must be float32 tensors on the scene's CUDA device")
+            if t.dim() != 2 or t.size(1) != 3 or t.size(0) < 1 or not t.is_contiguous():
+                raise RuntimeError("cmap_table entries must be contiguous [L, 3] tensors with L >= 1")
+        cached = getattr(self, "_cmap_cache", None)
+        if cached is not None and len(cached[0]) == 4 and all(
+                a is b and v == b._version for a, v, b in zip(cached[0], cached[1], tables)):
+            return cached[2], cached[3]
+        ptrs = torch.tensor([t.data_ptr() for t in tables], dtype=torch.int64).to(device)
+        sizes = torch.tensor([t.size(0) for t in tables], dtype=torch.int32).to(device)
+        self._cmap_cache = (tables, [t._version for t in tables], ptrs, sizes)
+        return ptrs, sizes
+
+    # Pipeline::trace_visualization (pipeline.h:102-115); the reference has no Python binding for it
+    def trace_visualization(self, points, attributes, point_adjacency, point_adjacency_offsets, adjacent_diff,
+                            camera, start_point, output_rgba=None, *, mode="rgb", color_map="turbo",
+                            cmap_table=None, bg_color=(1.0, 1.0, 1.0), checker_bg=False, max_depth=10.0,
+                            depth_quantile=0.5, weight_threshold=None, max_intersections=None):
+        """Preview frame of the foam seen by ``camera`` (the dict ``trace_benchmark`` takes), as RGBA8 words in a
+        uint32 ``[height, width]`` tensor whose rows are bottom-up, as on the reference's GL surface.
+
+        mode: "rgb" (colour over ``bg_color``, or a grey checker), "depth" (colormap of the depth where the
+        transmittance first falls below ``depth_quantile``, divided by ``max_depth``), "alpha" (1 - T), or
+        "intersections" (colormap of cells entered - 1 over ``max_intersections``).  ``cmap_table``: four float32
+        CUDA tensors ``[L_k, 3]`` indexed by colour map (gray, viridis, inferno, turbo); needed by "depth" and
+        "intersections" only.  ``start_point``: the entry cell, an int or a one-element uint32 tensor."""
+        if mode not in _lib.VIS_MODES:
+            raise RuntimeError(f"unknown visualization mode {mode!r}; one of {sorted(_lib.VIS_MODES)}")
+        if color_map not in _lib.COLOR_MAPS:
+            raise RuntimeError(f"unknown color map {color_map!r}; one of {sorted(_lib.COLOR_MAPS)}")
+        (points_c, attributes_c, adj_c, off_c), scene_key = self._scene_tensors(
+            points, attributes, point_adjacency, point_adjacency_offsets)
+        diff_c = adjacent_diff.contiguous()
+        num_points = points_c.size(0)
+        dev = points_c.device
+        cam = self._camera(camera)
+        if isinstance(start_point, torch.Tensor):
+            if start_point.numel() != 1:
+                raise RuntimeError("start_point must have a single element")
+            if start_point.dtype != torch.uint32:
+                raise RuntimeError("start_point must have uint32 dtype")
+            start = int(start_point.reshape(-1).cpu().numpy()[0])
+        else:
+            start = int(start_point)
+        if not 0 <= start < num_points:
+            raise RuntimeError("start_point must be a point of the scene")
+        if output_rgba is None:
+            output_rgba = torch.empty((cam.height, cam.width), dtype=torch.uint32, device=dev)
+        if output_rgba.numel() != cam.width * cam.height:
+            raise RuntimeError("output_rgba must have width * height elements")
+        if output_rgba.dtype != torch.uint32:
+            raise RuntimeError("output_rgba must have uint32 dtype")
+        if output_rgba.device != dev:
+            raise RuntimeError("output_rgba must be on the scene's CUDA device")
+        if not output_rgba.is_contiguous():
+            raise RuntimeError("output_rgba must be contiguous")
+        if diff_c.numel() * diff_c.element_size() < 8 * adj_c.numel():
+            raise RuntimeError("adjacent_diff must hold one half4 per adjacency entry")
+        table = _lib.CMapTable(None, None)
+        if mode in ("depth", "intersections"):
+            if cmap_table is None:
+                raise RuntimeError(f"mode {mode!r} needs a cmap_table")
+            ptrs, sizes = self._cmap_arrays(cmap_table, dev)
+            table = _lib.CMapTable(ptrs.data_ptr(), sizes.data_ptr())
+        vis = _lib.VisualizationSettings(_lib.VIS_MODES[mode], _lib.COLOR_MAPS[color_map],
+                                         (ctypes.c_float * 3)(*[float(c) for c in bg_color]), int(bool(checker_bg)),
+                                         float(max_depth), float(depth_quantile))
+        settings = self._settings(weight_threshold, max_intersections)
+        opts = self._opts(scene_key, None)
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            _lib.check(self._lib.rfb_trace_visualization_rgba8(
+                self._handle, ctypes.byref(settings), ctypes.byref(vis), ctypes.byref(cam), ctypes.byref(table),
+                num_points, 0, _ptr(points_c), _ptr(attributes_c), _ptr(adj_c), _ptr(off_c), _ptr(diff_c), start,
+                _ptr(output_rgba), ctypes.byref(opts), stream))
+        return output_rgba.view(cam.height, cam.width)
+
     # radfoam::prefetch_adjacent_diff (pipeline.h:50-56); handy for trace_benchmark callers
     def prefetch_adjacent_diff(self, points, point_adjacency, point_adjacency_offsets):
         points_c = points.contiguous()
