@@ -268,3 +268,17 @@ def test_emulated_kernels_small_scene_within_model_bounds(tape, monkeypatch):
     case = common.scene_case(num_points=1500, width=48, height=32, q=2)
     report = run_emu_case(case, np.float32, "cached", tape, monkeypatch)
     print("\n" + M.format_report(f"emu scene1500 tape={tape}", report))
+
+
+def test_compare_fp16_overflow_to_inf():
+    """An fp16 scatter entry whose sum reaches 65520 rounds to inf of its sign; a wrong sign, or inf where the bound
+    stays below the overflow, is still a mismatch."""
+    s = M.Scatter(3, 1)
+    s.add(np.array([0, 1, 2]), [0], M.EV(np.array([[7e4], [-7e4], [6e4]])))
+    s.flush()
+    m = {"ambiguous": np.zeros(0, dtype=bool), "attr_grad": s}
+    ok = np.array([[np.inf], [-np.inf], [6e4]], dtype=np.float16)
+    M.compare({"attr_grad": ok}, m, per_ray=False)
+    for bad in ([[-np.inf], [-np.inf], [6e4]], [[np.inf], [-np.inf], [np.inf]]):
+        with pytest.raises(M.Mismatch):
+            M.compare({"attr_grad": np.array(bad, dtype=np.float16)}, m, per_ray=False)
