@@ -239,6 +239,18 @@ __device__ __forceinline__ void normalize_dir(float &x, float &y, float &z) {
     z = __fdiv_rn(z, n);
 }
 
+// ray r of a [R][6] (origin, direction) array, its direction normalised
+__device__ __forceinline__ void load_ray(const float *rays, uint32_t r, RayGeom &ray) {
+    const float *rp = rays + 6 * (uint64_t)r;
+    ray.ox = __ldg(rp + 0);
+    ray.oy = __ldg(rp + 1);
+    ray.oz = __ldg(rp + 2);
+    ray.dx = __ldg(rp + 3);
+    ray.dy = __ldg(rp + 4);
+    ray.dz = __ldg(rp + 5);
+    normalize_dir(ray.dx, ray.dy, ray.dz);
+}
+
 // One bisector-plane test (tracing_utils.cuh:52-65).  `h` is one face record:
 // (dx, dy, dz, 0) in fp16 = RN_half(neighbour - cell point).  Association as in
 // the reference's SASS (SURVEY.md Appendix D, re-read from oracle/_ref):
@@ -599,6 +611,27 @@ __device__ __forceinline__ void sh_basis_grad(float x, float y, float z, const f
         acc(gx, __fmul_rn(3.0f, g15), __fsub_rn(xx, yy));
         acc(gy, __fmul_rn(-6.0f, g15), xy);
     }
+}
+
+// One composited cell of the forward-style kernels (forward cell functor, pipeline.cu:66-85): the cell's colour (its
+// SH row is read only above density 1e-6), alpha, the weight w = T alpha and the colour sums, in the association
+// every forward-style kernel pins.  `on_weight(w)` runs between the weight and the colour sums (the forward's
+// `contrib` atomics sit there).  Returns the transmittance behind the cell; T itself is left to the caller.
+template <int DEG, typename OnWeight>
+__device__ __forceinline__ float composite_cell(const float *__restrict__ sh_rows, const float *sh, uint32_t cell,
+                                                float s, float t0, float t1, float T, float &cr, float &cg,
+                                                float &cb, OnWeight &&on_weight) {
+    float r_ = 0.0f, g_ = 0.0f, b_ = 0.0f;
+    if (s > 1e-6f)
+        sh_to_rgb<DEG>(sh_rows + (uint64_t)cell * sh_row(DEG), sh, r_, g_, b_);
+    float delta = fmaxf(__fsub_rn(t1, t0), 0.0f);
+    float alpha = 1.0f - expf(-s * delta);
+    float w = __fmul_rn(T, alpha);
+    on_weight(w);
+    cr = __fmaf_rn(w, r_, cr);
+    cg = __fmaf_rn(w, g_, cg);
+    cb = __fmaf_rn(w, b_, cb);
+    return __fmul_rn(T, __fsub_rn(1.0f, alpha));
 }
 
 // Per-ray state of the backward pass and the analytic gradients of one composited cell

@@ -249,18 +249,9 @@ __global__ void __launch_bounds__(kBlock) forward_kernel(const ForwardParams p, 
         return;
 
     RayGeom ray;
-    {
-        const float *rp = p.rays + 6 * (uint64_t)r;
-        ray.ox = __ldg(rp + 0);
-        ray.oy = __ldg(rp + 1);
-        ray.oz = __ldg(rp + 2);
-        ray.dx = __ldg(rp + 3);
-        ray.dy = __ldg(rp + 4);
-        ray.dz = __ldg(rp + 5);
-        normalize_dir(ray.dx, ray.dy, ray.dz);
-        if (MODE == kScanFast && needs_exact_scan(ray.dx, ray.dy, ray.dz))
-            *p.exact_flag = 1u;
-    }
+    load_ray(p.rays, r, ray);
+    if (MODE == kScanFast && needs_exact_scan(ray.dx, ray.dy, ray.dz))
+        *p.exact_flag = 1u;
     float sh[sh_dim(DEG)];
     sh_basis<DEG>(ray.dx, ray.dy, ray.dz, sh);
 
@@ -273,23 +264,15 @@ __global__ void __launch_bounds__(kBlock) forward_kernel(const ForwardParams p, 
     float cr = 0.0f, cg = 0.0f, cb = 0.0f;
 
     auto cell_fn = [&](uint32_t cell, const float4 &pc, float t0, float t1, const float4 &) -> bool {
-        float s = pc.w;
-        float r_ = 0.0f, g_ = 0.0f, b_ = 0.0f;
-        if (s > 1e-6f)
-            sh_to_rgb<DEG>(p.sh_rows + (uint64_t)cell * sh_row(DEG), sh, r_, g_, b_);
-        float delta = fmaxf(__fsub_rn(t1, t0), 0.0f);
-        float alpha = 1.0f - expf(-s * delta);
-        float w = __fmul_rn(T, alpha);
-        if (p.contrib) {
-            if (p.out_half)
-                atomicAdd(reinterpret_cast<__half *>(p.contrib) + cell, __float2half_rn(w));
-            else
-                atomicAdd(reinterpret_cast<float *>(p.contrib) + cell, w);
-        }
-        cr = __fmaf_rn(w, r_, cr);
-        cg = __fmaf_rn(w, g_, cg);
-        cb = __fmaf_rn(w, b_, cb);
-        float Tn = __fmul_rn(T, __fsub_rn(1.0f, alpha));
+        const float s = pc.w;
+        const float Tn = composite_cell<DEG>(p.sh_rows, sh, cell, s, t0, t1, T, cr, cg, cb, [&](float w) {
+            if (p.contrib) {
+                if (p.out_half)
+                    atomicAdd(reinterpret_cast<__half *>(p.contrib) + cell, __float2half_rn(w));
+                else
+                    atomicAdd(reinterpret_cast<float *>(p.contrib) + cell, w);
+            }
+        });
         while (qi < Q && Tn < cq) {
             p.qdepth[(uint64_t)r * Q + qi] = __fadd_rn(t0, __fdiv_rn(logf(__fdiv_rn(T, cq)), s));
             p.qidx[(uint64_t)r * Q + qi] = cell;
@@ -493,14 +476,7 @@ __global__ void __launch_bounds__(kBlock) forward_record_kernel(const ForwardPar
     uint32_t cur = 0;
     float4 pc = make_float4(0.f, 0.f, 0.f, 0.f);
     if (has_ray) {
-        const float *rp = p.rays + 6 * (uint64_t)r;
-        ray.ox = __ldg(rp + 0);
-        ray.oy = __ldg(rp + 1);
-        ray.oz = __ldg(rp + 2);
-        ray.dx = __ldg(rp + 3);
-        ray.dy = __ldg(rp + 4);
-        ray.dz = __ldg(rp + 5);
-        normalize_dir(ray.dx, ray.dy, ray.dz);
+        load_ray(p.rays, r, ray);
         Q = p.quantiles ? p.num_q : 0u;
         qv = p.quantiles + (uint64_t)r * p.num_q;
         cq = Q ? __ldg(qv) : 0.0f;
@@ -552,6 +528,9 @@ __global__ void __launch_bounds__(kBlock) forward_record_kernel(const ForwardPar
                     uint32_t nxt = fa.neighbour(begin, face);
                     float4 pn = ldg4(p.cells + nxt);
                     if (t1 > t0) {
+                        // composite_cell() and forward_kernel's quantile loop, written out (as is the epilogue
+                        // below): shared, they move this kernel's register allocation and so its SASS.  Keep
+                        // these copies in step with forward_kernel.
                         float s = pc.w;
                         float r_ = 0.0f, g_ = 0.0f, b_ = 0.0f;
                         if (s > 1e-6f)
@@ -591,6 +570,7 @@ __global__ void __launch_bounds__(kBlock) forward_record_kernel(const ForwardPar
     if (!has_ray)
         return;
     tape.per_ray[r] = make_uint2(nrec, cur);
+    // forward_kernel's epilogue, written out (see the cell step above)
     while (qi < Q) {
         p.qdepth[(uint64_t)r * Q + qi] = -1.0f;
         p.qidx[(uint64_t)r * Q + qi] = kNone;
@@ -637,14 +617,7 @@ struct BackwardParams {
 template <int DEG>
 __device__ __forceinline__ void backward_ray_setup(const BackwardParams &p, uint32_t r, RayGeom &ray,
                                                    float *sh, BackwardRay &st) {
-    const float *rp = p.rays + 6 * (uint64_t)r;
-    ray.ox = __ldg(rp + 0);
-    ray.oy = __ldg(rp + 1);
-    ray.oz = __ldg(rp + 2);
-    ray.dx = __ldg(rp + 3);
-    ray.dy = __ldg(rp + 4);
-    ray.dz = __ldg(rp + 5);
-    normalize_dir(ray.dx, ray.dy, ray.dz);
+    load_ray(p.rays, r, ray);
     sh_basis<DEG>(ray.dx, ray.dy, ray.dz, sh);
     st.err = 0.0f;
     if (p.io_half) {
@@ -1536,17 +1509,7 @@ __global__ void __launch_bounds__(kBlock) benchmark_kernel(const BenchmarkParams
     sh_basis<DEG>(ray.dx, ray.dy, ray.dz, sh);
     float T = 1.0f, cr = 0.0f, cg = 0.0f, cb = 0.0f;
     auto cell_fn = [&](uint32_t cell, const float4 &pc, float t0, float t1, const float4 &) -> bool {
-        float s = pc.w;
-        float r_ = 0.0f, g_ = 0.0f, b_ = 0.0f;
-        if (s > 1e-6f)
-            sh_to_rgb<DEG>(p.sh_rows + (uint64_t)cell * sh_row(DEG), sh, r_, g_, b_);
-        float delta = fmaxf(__fsub_rn(t1, t0), 0.0f);
-        float alpha = 1.0f - expf(-s * delta);
-        float w = __fmul_rn(T, alpha);
-        cr = __fmaf_rn(w, r_, cr);
-        cg = __fmaf_rn(w, g_, cg);
-        cb = __fmaf_rn(w, b_, cb);
-        T = __fmul_rn(T, __fsub_rn(1.0f, alpha));
+        T = composite_cell<DEG>(p.sh_rows, sh, cell, pc.w, t0, t1, T, cr, cg, cb, [](float) {});
         return T > p.weight_threshold;
     };
     if (MODE == kScanFast && needs_exact_scan(ray.dx, ray.dy, ray.dz))
@@ -1684,17 +1647,8 @@ __global__ void __launch_bounds__(kBlock) visualization_kernel(const Visualizati
     float depth = 0.0f;
     bool passed = false;
     auto cell_fn = [&](uint32_t cell, const float4 &pc, float t0, float t1, const float4 &) -> bool {
-        float s = pc.w;
-        float r_ = 0.0f, g_ = 0.0f, b_ = 0.0f;
-        if (s > 1e-6f)
-            sh_to_rgb<DEG>(p.sh_rows + (uint64_t)cell * sh_row(DEG), sh, r_, g_, b_);
-        float delta = fmaxf(__fsub_rn(t1, t0), 0.0f);
-        float alpha = 1.0f - expf(-s * delta);
-        float w = __fmul_rn(T, alpha);
-        cr = __fmaf_rn(w, r_, cr);
-        cg = __fmaf_rn(w, g_, cg);
-        cb = __fmaf_rn(w, b_, cb);
-        float Tn = __fmul_rn(T, __fsub_rn(1.0f, alpha));
+        const float s = pc.w;
+        const float Tn = composite_cell<DEG>(p.sh_rows, sh, cell, s, t0, t1, T, cr, cg, cb, [](float) {});
         if (!passed && Tn < q) { // the forward's quantile depth, first quantile only
             depth = __fadd_rn(t0, __fdiv_rn(logf(__fdiv_rn(T, q)), s));
             passed = true;

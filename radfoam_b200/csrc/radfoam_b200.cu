@@ -12,6 +12,7 @@
 #include <cstring>
 #include <new>
 #include <string>
+#include <type_traits>
 
 #include "foam_kernels.cuh"
 
@@ -101,6 +102,39 @@ int grid_for(uint64_t work_items, int block, int max_blocks = kNumSMs * 16) {
     if (b < 1)
         b = 1;
     return (int)b;
+}
+
+// f(std::integral_constant<int, D>{}) for SH degree D: one kernel instantiation per degree
+template <typename F>
+auto with_degree(int deg, F &&f) {
+    switch (deg) {
+    case 0: return f(std::integral_constant<int, 0>{});
+    case 1: return f(std::integral_constant<int, 1>{});
+    case 2: return f(std::integral_constant<int, 2>{});
+    default: return f(std::integral_constant<int, 3>{});
+    }
+}
+
+template <typename T>
+struct TypeTag {
+    using type = T;
+};
+
+// f(TypeTag<AttrT>{}) for the attribute dtype: __half for RFB_FLOAT16, else float
+template <typename F>
+auto with_attr_type(int attr_dtype, F &&f) {
+    if (attr_dtype == RFB_FLOAT16)
+        return f(TypeTag<__half>{});
+    return f(TypeTag<float>{});
+}
+
+// The fast kernel and, right behind it, its exact twin (a no-op unless the fast one raised the flag);
+// launch(std::integral_constant<int, MODE>{}) launches one of them.
+template <typename F>
+int launch_twins(F &&launch) {
+    if (int rc = launch(std::integral_constant<int, rfb::kScanFast>{}))
+        return rc;
+    return launch(std::integral_constant<int, rfb::kScanExactTwin>{});
 }
 
 } // namespace
@@ -260,42 +294,24 @@ int ensure_scene(rfb_pipeline *p, uint32_t n, const float *points, const void *a
     if (n && p->params_bound) {
         const int grid = grid_for((uint64_t)n * (SR / 4), 256 * 4, kNumSMs * 8);
         float4 *cells = reinterpret_cast<float4 *>(p->cells.ptr), *rows = reinterpret_cast<float4 *>(p->sh_rows.ptr);
-#define RFB_BUILD_PARAMS(DEG)                                                                                      \
-    do {                                                                                                           \
-        if (p->attr_dtype == RFB_FLOAT16)                                                                          \
-            RFB_LAUNCH((build_cells_params_kernel<__half, DEG>), grid, 256, 0, stream, points, p->params.att_dc,   \
-                       p->params.att_sh, p->params.density, p->params.activation_scale, n, cells, rows);           \
-        else                                                                                                       \
-            RFB_LAUNCH((build_cells_params_kernel<float, DEG>), grid, 256, 0, stream, points, p->params.att_dc,    \
-                       p->params.att_sh, p->params.density, p->params.activation_scale, n, cells, rows);           \
-    } while (0)
-        switch (p->sh_degree) {
-        case 0: RFB_BUILD_PARAMS(0); break;
-        case 1: RFB_BUILD_PARAMS(1); break;
-        case 2: RFB_BUILD_PARAMS(2); break;
-        default: RFB_BUILD_PARAMS(3); break;
-        }
-#undef RFB_BUILD_PARAMS
+        with_degree(p->sh_degree, [&](auto d) {
+            with_attr_type(p->attr_dtype, [&](auto t) {
+                RFB_LAUNCH((build_cells_params_kernel<typename decltype(t)::type, decltype(d)::value>), grid, 256, 0,
+                           stream, points, p->params.att_dc, p->params.att_sh, p->params.density,
+                           p->params.activation_scale, n, cells, rows);
+            });
+        });
         RFB_LAUNCHED();
     } else if (n) {
         const int grid = grid_for((uint64_t)n * (SR / 4), 256 * 4, kNumSMs * 8);
         float4 *cells = reinterpret_cast<float4 *>(p->cells.ptr), *rows = reinterpret_cast<float4 *>(p->sh_rows.ptr);
-#define RFB_BUILD_CELLS(DEG)                                                                                       \
-    do {                                                                                                           \
-        if (p->attr_dtype == RFB_FLOAT16)                                                                          \
-            RFB_LAUNCH((build_cells_kernel<__half, DEG>), grid, 256, 0, stream, points,                            \
-                       reinterpret_cast<const __half *>(attrs), n, cells, rows);                                   \
-        else                                                                                                       \
-            RFB_LAUNCH((build_cells_kernel<float, DEG>), grid, 256, 0, stream, points,                             \
-                       reinterpret_cast<const float *>(attrs), n, cells, rows);                                    \
-    } while (0)
-        switch (p->sh_degree) {
-        case 0: RFB_BUILD_CELLS(0); break;
-        case 1: RFB_BUILD_CELLS(1); break;
-        case 2: RFB_BUILD_CELLS(2); break;
-        default: RFB_BUILD_CELLS(3); break;
-        }
-#undef RFB_BUILD_CELLS
+        with_degree(p->sh_degree, [&](auto d) {
+            with_attr_type(p->attr_dtype, [&](auto t) {
+                using AttrT = typename decltype(t)::type;
+                RFB_LAUNCH((build_cells_kernel<AttrT, decltype(d)::value>), grid, 256, 0, stream, points,
+                           reinterpret_cast<const AttrT *>(attrs), n, cells, rows);
+            });
+        });
         RFB_LAUNCHED();
     }
     if (need_faces) {
@@ -344,50 +360,63 @@ int profile_mark(rfb_pipeline *p, int which, cudaStream_t stream) {
     return 0;
 }
 
-template <typename Faces, int MODE>
-int launch_forward_mode(int deg, const ForwardParams &fp, const Faces &fa, uint32_t blocks, cudaStream_t stream) {
-    switch (deg) {
-    case 0: RFB_LAUNCH((forward_kernel<0, Faces, MODE>), blocks, kBlock, 0, stream, fp, fa); break;
-    case 1: RFB_LAUNCH((forward_kernel<1, Faces, MODE>), blocks, kBlock, 0, stream, fp, fa); break;
-    case 2: RFB_LAUNCH((forward_kernel<2, Faces, MODE>), blocks, kBlock, 0, stream, fp, fa); break;
-    default: RFB_LAUNCH((forward_kernel<3, Faces, MODE>), blocks, kBlock, 0, stream, fp, fa); break;
-    }
-    RFB_LAUNCHED();
-    return 0;
-}
-
-// The fast kernel and, right behind it, its exact twin (a no-op unless the fast one raised the flag); with a
-// contribution output (accumulated by atomics: a second pass would double it) one launch that chooses per ray.
 template <typename Faces>
 int launch_forward(int deg, const ForwardParams &fp, const Faces &fa, uint32_t blocks, cudaStream_t stream) {
-    if (fp.contrib)
-        return launch_forward_mode<Faces, kScanPerRay>(deg, fp, fa, blocks, stream);
-    if (int rc = launch_forward_mode<Faces, kScanFast>(deg, fp, fa, blocks, stream))
-        return rc;
-    return launch_forward_mode<Faces, kScanExactTwin>(deg, fp, fa, blocks, stream);
-}
-
-template <typename Faces, int MODE>
-int launch_forward_record_mode(int deg, const ForwardParams &fp, const Faces &fa, const Tape &tape, uint32_t blocks,
-                               cudaStream_t stream) {
-    switch (deg) {
-    case 0: RFB_LAUNCH((forward_record_kernel<0, Faces, MODE>), blocks, kBlock, 0, stream, fp, fa, tape); break;
-    case 1: RFB_LAUNCH((forward_record_kernel<1, Faces, MODE>), blocks, kBlock, 0, stream, fp, fa, tape); break;
-    case 2: RFB_LAUNCH((forward_record_kernel<2, Faces, MODE>), blocks, kBlock, 0, stream, fp, fa, tape); break;
-    default: RFB_LAUNCH((forward_record_kernel<3, Faces, MODE>), blocks, kBlock, 0, stream, fp, fa, tape); break;
-    }
-    RFB_LAUNCHED();
-    return 0;
+    auto launch = [&](auto mode) {
+        return with_degree(deg, [&](auto d) {
+            RFB_LAUNCH((forward_kernel<decltype(d)::value, Faces, decltype(mode)::value>), blocks, kBlock, 0, stream,
+                       fp, fa);
+            RFB_LAUNCHED();
+            return 0;
+        });
+    };
+    // with a contribution output (accumulated by atomics: a second pass would double it) one launch that chooses
+    // per ray
+    return fp.contrib ? launch(std::integral_constant<int, kScanPerRay>{}) : launch_twins(launch);
 }
 
 template <typename Faces>
 int launch_forward_record(int deg, const ForwardParams &fp, const Faces &fa, const Tape &tape,
                           uint32_t blocks, cudaStream_t stream) {
-    if (fp.contrib)
-        return launch_forward_record_mode<Faces, kScanPerRay>(deg, fp, fa, tape, blocks, stream);
-    if (int rc = launch_forward_record_mode<Faces, kScanFast>(deg, fp, fa, tape, blocks, stream))
-        return rc;
-    return launch_forward_record_mode<Faces, kScanExactTwin>(deg, fp, fa, tape, blocks, stream);
+    auto launch = [&](auto mode) {
+        return with_degree(deg, [&](auto d) {
+            RFB_LAUNCH((forward_record_kernel<decltype(d)::value, Faces, decltype(mode)::value>), blocks, kBlock, 0,
+                       stream, fp, fa, tape);
+            RFB_LAUNCHED();
+            return 0;
+        });
+    };
+    return fp.contrib ? launch(std::integral_constant<int, kScanPerRay>{}) : launch_twins(launch);
+}
+
+// The device view of the pipeline's tape buffers; `order` (the replay schedule) is left to the caller.
+Tape pipeline_tape(const rfb_pipeline *p) {
+    Tape tape = {};
+    tape.pool = reinterpret_cast<uint2 *>(p->tape_pool.ptr);
+    tape.table = reinterpret_cast<uint32_t *>(p->tape_table.ptr);
+    tape.per_ray = reinterpret_cast<uint2 *>(p->tape_per_ray.ptr);
+    tape.ctrl = reinterpret_cast<uint32_t *>(p->tape_ctrl.ptr);
+    tape.capacity = p->tape_capacity;
+    tape.table_stride = p->tape_table_stride;
+    tape.tile_steps = reinterpret_cast<uint32_t *>(p->tape_sched.ptr);
+    return tape;
+}
+
+// The walk's view of the pipeline's face mirror, with the caller's CSR offsets.
+PaddedFaces padded_faces(const rfb_pipeline *p, const uint32_t *offsets) {
+    PaddedFaces fa;
+    fa.faces = reinterpret_cast<const uint2 *>(p->faces.ptr);
+    fa.nbr = reinterpret_cast<const uint32_t *>(p->nbr.ptr);
+    fa.off = offsets;
+    return fa;
+}
+
+// Clears the exact-scan flag (ScanMode) a fast kernel raises for its twin and points `flag` at it.
+int reset_exact_flag(rfb_pipeline *p, cudaStream_t stream, uint32_t *&flag) {
+    RFB_CUDA(p->scan_flag.ensure(4 * sizeof(uint32_t)));
+    RFB_CUDA(cudaMemsetAsync(p->scan_flag.ptr, 0, 4 * sizeof(uint32_t), stream));
+    flag = reinterpret_cast<uint32_t *>(p->scan_flag.ptr);
+    return 0;
 }
 
 // Size / reset the tape for a recording forward of `blocks` CTAs; fills `tape`.  The tape is an optimisation:
@@ -435,41 +464,29 @@ int prepare_tape(rfb_pipeline *p, uint32_t blocks, uint32_t num_rays, uint32_t m
     }
     RFB_CUDA(cudaMemsetAsync(p->tape_ctrl.ptr, 0, 4 * sizeof(uint32_t), stream));
     p->tape_blocks = blocks;
-    tape.tile_steps = reinterpret_cast<uint32_t *>(p->tape_sched.ptr);
-    tape.order = tape.tile_steps + blocks;
     if (!p->tape_readback) {
         RFB_CUDA(cudaMallocHost(reinterpret_cast<void **>(&p->tape_readback), 4 * sizeof(uint32_t)));
         RFB_CUDA(cudaEventCreateWithFlags(&p->tape_readback_done, cudaEventDisableTiming));
     }
     p->tape_table_stride = stride;
-    tape.pool = reinterpret_cast<uint2 *>(p->tape_pool.ptr);
-    tape.table = reinterpret_cast<uint32_t *>(p->tape_table.ptr);
-    tape.per_ray = reinterpret_cast<uint2 *>(p->tape_per_ray.ptr);
-    tape.ctrl = reinterpret_cast<uint32_t *>(p->tape_ctrl.ptr);
-    tape.capacity = p->tape_capacity;
-    tape.table_stride = stride;
+    tape = pipeline_tape(p);
+    tape.order = tape.tile_steps + blocks;
     ok = true;
-    return 0;
-}
-
-template <typename Faces, bool RAY>
-int launch_backward_ray(int deg, const BackwardParams &bp, const Faces &fa, const RayGradOut &rg, uint32_t blocks,
-                        cudaStream_t stream) {
-    switch (deg) {
-    case 0: RFB_LAUNCH((backward_kernel<0, Faces, RAY>), blocks, kBlock, 0, stream, bp, fa, rg); break;
-    case 1: RFB_LAUNCH((backward_kernel<1, Faces, RAY>), blocks, kBlock, 0, stream, bp, fa, rg); break;
-    case 2: RFB_LAUNCH((backward_kernel<2, Faces, RAY>), blocks, kBlock, 0, stream, bp, fa, rg); break;
-    default: RFB_LAUNCH((backward_kernel<3, Faces, RAY>), blocks, kBlock, 0, stream, bp, fa, rg); break;
-    }
-    RFB_LAUNCHED();
     return 0;
 }
 
 template <typename Faces>
 int launch_backward(int deg, const BackwardParams &bp, const Faces &fa, const RayGradOut &rg, uint32_t blocks,
                     cudaStream_t stream) {
-    return rg.ray_grad ? launch_backward_ray<Faces, true>(deg, bp, fa, rg, blocks, stream)
-                       : launch_backward_ray<Faces, false>(deg, bp, fa, rg, blocks, stream);
+    auto launch = [&](auto ray) {
+        return with_degree(deg, [&](auto d) {
+            RFB_LAUNCH((backward_kernel<decltype(d)::value, Faces, decltype(ray)::value>), blocks, kBlock, 0, stream,
+                       bp, fa, rg);
+            RFB_LAUNCHED();
+            return 0;
+        });
+    };
+    return rg.ray_grad ? launch(std::true_type{}) : launch(std::false_type{});
 }
 
 template <int DEG, typename Faces, int SLOTS, int MIN_GROUP, int MIN_BLOCKS, bool REPLAY, bool RAY>
@@ -514,62 +531,43 @@ int launch_backward_cached_cfg(const BackwardParams &bp, const Faces &fa, const 
 // (<= 168) for degree 3, which spills at 128.
 template <int DEG, bool RAY>
 constexpr int backward_min_blocks() { return !RAY ? 5 : DEG == 3 ? 3 : 4; }
-template <typename Faces, bool RAY>
-int launch_backward_cached_ray(int deg, const BackwardParams &bp, const Faces &fa, const Tape &tape,
-                               const RayGradOut &rg, uint32_t blocks, cudaStream_t stream) {
-    switch (deg) {
-    case 0: return launch_backward_cached_cfg<0, Faces, 4, 6, backward_min_blocks<0, RAY>(), RAY>(bp, fa, tape, rg, blocks, stream);
-    case 1: return launch_backward_cached_cfg<1, Faces, 4, 6, backward_min_blocks<1, RAY>(), RAY>(bp, fa, tape, rg, blocks, stream);
-    case 2: return launch_backward_cached_cfg<2, Faces, 4, 6, backward_min_blocks<2, RAY>(), RAY>(bp, fa, tape, rg, blocks, stream);
-    default: return launch_backward_cached_cfg<3, Faces, 4, 6, backward_min_blocks<3, RAY>(), RAY>(bp, fa, tape, rg, blocks, stream);
-    }
-}
-
 template <typename Faces>
 int launch_backward_cached(int deg, const BackwardParams &bp, const Faces &fa, const Tape &tape,
                            const RayGradOut &rg, uint32_t blocks, cudaStream_t stream) {
-    return rg.ray_grad ? launch_backward_cached_ray<Faces, true>(deg, bp, fa, tape, rg, blocks, stream)
-                       : launch_backward_cached_ray<Faces, false>(deg, bp, fa, tape, rg, blocks, stream);
-}
-
-template <typename Faces, int MODE>
-int launch_benchmark_mode(int deg, const BenchmarkParams &bp, const Faces &fa, uint32_t blocks, cudaStream_t stream) {
-    switch (deg) {
-    case 0: RFB_LAUNCH((benchmark_kernel<0, Faces, MODE>), blocks, kBlock, 0, stream, bp, fa); break;
-    case 1: RFB_LAUNCH((benchmark_kernel<1, Faces, MODE>), blocks, kBlock, 0, stream, bp, fa); break;
-    case 2: RFB_LAUNCH((benchmark_kernel<2, Faces, MODE>), blocks, kBlock, 0, stream, bp, fa); break;
-    default: RFB_LAUNCH((benchmark_kernel<3, Faces, MODE>), blocks, kBlock, 0, stream, bp, fa); break;
-    }
-    RFB_LAUNCHED();
-    return 0;
+    auto launch = [&](auto ray) {
+        return with_degree(deg, [&](auto d) {
+            constexpr int DEG = decltype(d)::value;
+            constexpr bool RAY = decltype(ray)::value;
+            return launch_backward_cached_cfg<DEG, Faces, 4, 6, backward_min_blocks<DEG, RAY>(), RAY>(bp, fa, tape, rg,
+                                                                                                  blocks, stream);
+        });
+    };
+    return rg.ray_grad ? launch(std::true_type{}) : launch(std::false_type{});
 }
 
 template <typename Faces>
 int launch_benchmark(int deg, const BenchmarkParams &bp, const Faces &fa, uint32_t blocks, cudaStream_t stream) {
-    if (int rc = launch_benchmark_mode<Faces, kScanFast>(deg, bp, fa, blocks, stream))
-        return rc;
-    return launch_benchmark_mode<Faces, kScanExactTwin>(deg, bp, fa, blocks, stream);
-}
-
-template <typename Faces, int MODE, typename Out>
-int launch_visualization_mode(int deg, const VisualizationParams &vp, const Faces &fa, const Out &out,
-                              uint32_t blocks, cudaStream_t stream) {
-    switch (deg) {
-    case 0: RFB_LAUNCH((visualization_kernel<0, Faces, MODE, Out>), blocks, kBlock, 0, stream, vp, fa, out); break;
-    case 1: RFB_LAUNCH((visualization_kernel<1, Faces, MODE, Out>), blocks, kBlock, 0, stream, vp, fa, out); break;
-    case 2: RFB_LAUNCH((visualization_kernel<2, Faces, MODE, Out>), blocks, kBlock, 0, stream, vp, fa, out); break;
-    default: RFB_LAUNCH((visualization_kernel<3, Faces, MODE, Out>), blocks, kBlock, 0, stream, vp, fa, out); break;
-    }
-    RFB_LAUNCHED();
-    return 0;
+    return launch_twins([&](auto mode) {
+        return with_degree(deg, [&](auto d) {
+            RFB_LAUNCH((benchmark_kernel<decltype(d)::value, Faces, decltype(mode)::value>), blocks, kBlock, 0, stream,
+                       bp, fa);
+            RFB_LAUNCHED();
+            return 0;
+        });
+    });
 }
 
 template <typename Faces, typename Out>
 int launch_visualization(int deg, const VisualizationParams &vp, const Faces &fa, const Out &out, uint32_t blocks,
                          cudaStream_t stream) {
-    if (int rc = launch_visualization_mode<Faces, kScanFast>(deg, vp, fa, out, blocks, stream))
-        return rc;
-    return launch_visualization_mode<Faces, kScanExactTwin>(deg, vp, fa, out, blocks, stream);
+    return launch_twins([&](auto mode) {
+        return with_degree(deg, [&](auto d) {
+            RFB_LAUNCH((visualization_kernel<decltype(d)::value, Faces, decltype(mode)::value, Out>), blocks, kBlock,
+                       0, stream, vp, fa, out);
+            RFB_LAUNCHED();
+            return 0;
+        });
+    });
 }
 
 rfb_trace_settings settings_or_default(const rfb_trace_settings *s) {
@@ -667,16 +665,11 @@ int trace_visualization(const char *fn, rfb_pipeline *p, const rfb_trace_setting
     vp.depth_quantile = vis->depth_quantile;
     vp.cmap.data = uses_cmap ? cmap_table->data : nullptr;
     vp.cmap.sizes = uses_cmap ? cmap_table->sizes : nullptr;
-    RFB_CUDA(p->scan_flag.ensure(4 * sizeof(uint32_t)));
-    RFB_CUDA(cudaMemsetAsync(p->scan_flag.ptr, 0, 4 * sizeof(uint32_t), stream));
-    vp.exact_flag = reinterpret_cast<uint32_t *>(p->scan_flag.ptr);
+    if (int rc = reset_exact_flag(p, stream, vp.exact_flag))
+        return rc;
     vp.blocks_x = (camera->width + kTileW - 1) / kTileW;
     uint32_t blocks = vp.blocks_x * ((camera->height + kTileH - 1) / kTileH);
-    PaddedFaces fa;
-    fa.faces = reinterpret_cast<const uint2 *>(p->faces.ptr);
-    fa.nbr = reinterpret_cast<const uint32_t *>(p->nbr.ptr);
-    fa.off = point_adjacency_offsets;
-    return launch_visualization(p->sh_degree, vp, fa, out, blocks, stream);
+    return launch_visualization(p->sh_degree, vp, padded_faces(p, point_adjacency_offsets), out, blocks, stream);
 }
 
 } // namespace
@@ -941,13 +934,9 @@ int rfb_trace_forward(rfb_pipeline *p, const rfb_trace_settings *settings, uint3
     fp.out_half = p->attr_dtype == RFB_FLOAT16;
     uint32_t blocks;
     ray_grid(num_rays, opts ? opts->image_width : 0, blocks, fp.blocks_x, fp.image_width);
-    PaddedFaces fa;
-    fa.faces = reinterpret_cast<const uint2 *>(p->faces.ptr);
-    fa.nbr = reinterpret_cast<const uint32_t *>(p->nbr.ptr);
-    fa.off = point_adjacency_offsets;
-    RFB_CUDA(p->scan_flag.ensure(4 * sizeof(uint32_t)));
-    RFB_CUDA(cudaMemsetAsync(p->scan_flag.ptr, 0, 4 * sizeof(uint32_t), stream));
-    fp.exact_flag = reinterpret_cast<uint32_t *>(p->scan_flag.ptr);
+    const PaddedFaces fa = padded_faces(p, point_adjacency_offsets);
+    if (int rc = reset_exact_flag(p, stream, fp.exact_flag))
+        return rc;
     bool record = opts && (opts->flags & RFB_FLAG_RECORD_TAPE) && opts->scene_version != 0;
     p->tape_valid = false;
     Tape tape = {};
@@ -1070,10 +1059,7 @@ int rfb_trace_backward_accumulate_rays(rfb_pipeline *p, const rfb_trace_settings
     bp.io_half = p->attr_dtype == RFB_FLOAT16;
     uint32_t blocks;
     ray_grid(num_rays, opts ? opts->image_width : 0, blocks, bp.blocks_x, bp.image_width);
-    PaddedFaces fa;
-    fa.faces = reinterpret_cast<const uint2 *>(p->faces.ptr);
-    fa.nbr = reinterpret_cast<const uint32_t *>(p->nbr.ptr);
-    fa.off = point_adjacency_offsets;
+    const PaddedFaces fa = padded_faces(p, point_adjacency_offsets);
     if (int rc = profile_mark(p, 2, stream))
         return rc;
     const char *mode = getenv("RFB_BWD_MODE"); // "direct" | "cached" (experiment switch)
@@ -1086,13 +1072,7 @@ int rfb_trace_backward_accumulate_rays(rfb_pipeline *p, const rfb_trace_settings
         tk.scene_version == opts->scene_version && tk.rays == rays && tk.start == start_point_index &&
         tk.num_rays == num_rays && tk.image_width == bp.image_width && tk.max_steps == s.max_intersections &&
         tk.weight_threshold == s.weight_threshold) {
-        tape.pool = reinterpret_cast<uint2 *>(p->tape_pool.ptr);
-        tape.table = reinterpret_cast<uint32_t *>(p->tape_table.ptr);
-        tape.per_ray = reinterpret_cast<uint2 *>(p->tape_per_ray.ptr);
-        tape.ctrl = reinterpret_cast<uint32_t *>(p->tape_ctrl.ptr);
-        tape.capacity = p->tape_capacity;
-        tape.table_stride = p->tape_table_stride;
-        tape.tile_steps = reinterpret_cast<uint32_t *>(p->tape_sched.ptr);
+        tape = pipeline_tape(p);
         tape.order = (blocks == p->tape_blocks && p->tape_scheduled) ? tape.tile_steps + blocks : nullptr;
         if (int rc = wait_for(p->tape_ready, p->tape_stream, stream))
             return rc;
@@ -1170,31 +1150,18 @@ int rfb_reduce_finalize_peers(rfb_pipeline *p, uint32_t world, uint32_t rank, ui
         return 0;
     int grid = (int)(mine < kNumSMs * 16u ? mine : kNumSMs * 16u);
     cudaStream_t stream = (cudaStream_t)stream_;
-    const bool half = p->attr_dtype == RFB_FLOAT16;
-#define RFB_PEER_LAUNCH(DEG, W)                                                                          \
-    do {                                                                                                 \
-        if (half)                                                                                        \
-            RFB_LAUNCH((reduce_finalize_peers_kernel<DEG, __half, W>), grid, 256, 0, stream, pr);        \
-        else                                                                                             \
-            RFB_LAUNCH((reduce_finalize_peers_kernel<DEG, float, W>), grid, 256, 0, stream, pr);         \
-    } while (0)
-#define RFB_PEER_WORLD(DEG)                                                                              \
-    do {                                                                                                 \
-        switch (world) {                                                                                 \
-        case 2: RFB_PEER_LAUNCH(DEG, 2); break;                                                          \
-        case 4: RFB_PEER_LAUNCH(DEG, 4); break;                                                          \
-        case 8: RFB_PEER_LAUNCH(DEG, 8); break;                                                          \
-        default: RFB_PEER_LAUNCH(DEG, 0); break;                                                         \
-        }                                                                                                \
-    } while (0)
-    switch (p->sh_degree) {
-    case 0: RFB_PEER_WORLD(0); break;
-    case 1: RFB_PEER_WORLD(1); break;
-    case 2: RFB_PEER_WORLD(2); break;
-    default: RFB_PEER_WORLD(3); break;
-    }
-#undef RFB_PEER_WORLD
-#undef RFB_PEER_LAUNCH
+    with_degree(p->sh_degree, [&](auto d) {
+        with_attr_type(p->attr_dtype, [&](auto t) {
+            constexpr int DEG = decltype(d)::value;
+            using AttrT = typename decltype(t)::type;
+            switch (world) {
+            case 2: RFB_LAUNCH((reduce_finalize_peers_kernel<DEG, AttrT, 2>), grid, 256, 0, stream, pr); break;
+            case 4: RFB_LAUNCH((reduce_finalize_peers_kernel<DEG, AttrT, 4>), grid, 256, 0, stream, pr); break;
+            case 8: RFB_LAUNCH((reduce_finalize_peers_kernel<DEG, AttrT, 8>), grid, 256, 0, stream, pr); break;
+            default: RFB_LAUNCH((reduce_finalize_peers_kernel<DEG, AttrT, 0>), grid, 256, 0, stream, pr); break;
+            }
+        });
+    });
     RFB_LAUNCHED();
     return 0;
 }
@@ -1214,22 +1181,13 @@ int rfb_trace_backward_finalize(rfb_pipeline *p, uint32_t num_points, float *poi
     const int grid = grid_for((uint64_t)num_points * A, 256 * 4, kNumSMs * 8);
     int scrub = (flags & RFB_FLAG_SCRUB_NONFINITE) ? 1 : 0;
     const float *acc_ptr = p->acc_external ? p->acc_external : reinterpret_cast<const float *>(p->acc.ptr);
-#define RFB_FINALIZE(DEG)                                                                                          \
-    do {                                                                                                           \
-        if (p->attr_dtype == RFB_FLOAT16)                                                                          \
-            RFB_LAUNCH((finalize_grads_kernel<__half, DEG>), grid, 256, 0, stream, acc_ptr, num_points,            \
-                       points_grad, reinterpret_cast<__half *>(attribute_grad), scrub);                            \
-        else                                                                                                       \
-            RFB_LAUNCH((finalize_grads_kernel<float, DEG>), grid, 256, 0, stream, acc_ptr, num_points,             \
-                       points_grad, reinterpret_cast<float *>(attribute_grad), scrub);                             \
-    } while (0)
-    switch (p->sh_degree) {
-    case 0: RFB_FINALIZE(0); break;
-    case 1: RFB_FINALIZE(1); break;
-    case 2: RFB_FINALIZE(2); break;
-    default: RFB_FINALIZE(3); break;
-    }
-#undef RFB_FINALIZE
+    with_degree(p->sh_degree, [&](auto d) {
+        with_attr_type(p->attr_dtype, [&](auto t) {
+            using AttrT = typename decltype(t)::type;
+            RFB_LAUNCH((finalize_grads_kernel<AttrT, decltype(d)::value>), grid, 256, 0, stream, acc_ptr, num_points,
+                       points_grad, reinterpret_cast<AttrT *>(attribute_grad), scrub);
+        });
+    });
     RFB_LAUNCHED();
     return 0;
 }
@@ -1267,24 +1225,13 @@ int rfb_trace_backward_finalize_params(rfb_pipeline *p, uint32_t num_points, flo
     const int grid = grid_for((uint64_t)num_points * A, 256 * 4, kNumSMs * 8);
     int scrub = (flags & RFB_FLAG_SCRUB_NONFINITE) ? 1 : 0;
     const float *acc_ptr = p->acc_external ? p->acc_external : reinterpret_cast<const float *>(p->acc.ptr);
-#define RFB_FINALIZE_PARAMS(DEG)                                                                                   \
-    do {                                                                                                           \
-        if (p->attr_dtype == RFB_FLOAT16)                                                                          \
-            RFB_LAUNCH((finalize_params_kernel<__half, DEG>), grid, 256, 0, stream, acc_ptr, p->params.density,    \
-                       p->params.activation_scale, num_points, points_grad, att_dc_grad, att_sh_grad,              \
-                       density_grad, scrub);                                                                       \
-        else                                                                                                       \
-            RFB_LAUNCH((finalize_params_kernel<float, DEG>), grid, 256, 0, stream, acc_ptr, p->params.density,     \
-                       p->params.activation_scale, num_points, points_grad, att_dc_grad, att_sh_grad,              \
-                       density_grad, scrub);                                                                       \
-    } while (0)
-    switch (p->sh_degree) {
-    case 0: RFB_FINALIZE_PARAMS(0); break;
-    case 1: RFB_FINALIZE_PARAMS(1); break;
-    case 2: RFB_FINALIZE_PARAMS(2); break;
-    default: RFB_FINALIZE_PARAMS(3); break;
-    }
-#undef RFB_FINALIZE_PARAMS
+    with_degree(p->sh_degree, [&](auto d) {
+        with_attr_type(p->attr_dtype, [&](auto t) {
+            RFB_LAUNCH((finalize_params_kernel<typename decltype(t)::type, decltype(d)::value>), grid, 256, 0, stream,
+                       acc_ptr, p->params.density, p->params.activation_scale, num_points, points_grad, att_dc_grad,
+                       att_sh_grad, density_grad, scrub);
+        });
+    });
     RFB_LAUNCHED();
     return 0;
 }
@@ -1342,17 +1289,12 @@ int rfb_trace_benchmark(rfb_pipeline *p, const rfb_trace_settings *settings, uin
     bp.cam = camera_params(camera);
     bp.weight_threshold = s.weight_threshold;
     bp.max_steps = s.max_intersections;
-    RFB_CUDA(p->scan_flag.ensure(4 * sizeof(uint32_t)));
-    RFB_CUDA(cudaMemsetAsync(p->scan_flag.ptr, 0, 4 * sizeof(uint32_t), stream));
-    bp.exact_flag = reinterpret_cast<uint32_t *>(p->scan_flag.ptr);
+    if (int rc = reset_exact_flag(p, stream, bp.exact_flag))
+        return rc;
     bp.blocks_x = (camera->width + kTileW - 1) / kTileW;
     uint32_t blocks = bp.blocks_x * ((camera->height + kTileH - 1) / kTileH);
     // the caller's offsets, re-laid-out (copied, not recomputed) into the padded face rows
-    PaddedFaces fa;
-    fa.faces = reinterpret_cast<const uint2 *>(p->faces.ptr);
-    fa.nbr = reinterpret_cast<const uint32_t *>(p->nbr.ptr);
-    fa.off = point_adjacency_offsets;
-    return launch_benchmark(p->sh_degree, bp, fa, blocks, stream);
+    return launch_benchmark(p->sh_degree, bp, padded_faces(p, point_adjacency_offsets), blocks, stream);
 }
 
 int rfb_trace_visualization(rfb_pipeline *p, const rfb_trace_settings *settings,
