@@ -12,6 +12,8 @@
  *   rfb_trace_backward       <- Pipeline::trace_backward            src/tracing/pipeline.h:80-100
  *   rfb_trace_benchmark      <- Pipeline::trace_benchmark           src/tracing/pipeline.h:117-126
  *   rfb_trace_visualization <- Pipeline::trace_visualization src/tracing/pipeline.h:102-115
+ *   rfb_locate_points        <- radfoam::nn over the AABB tree  src/aabb_tree/aabb_tree.cu:343-415 (any number of queries)
+ *   rfb_sample_field(_backward)  (new) the field at arbitrary points and its attribute gradient
  *
  * The reference interface is a C++ vtable taking raw device pointers (Eigen
  * types appear only as reinterpret_casts of packed floats); this header
@@ -152,7 +154,7 @@ int rfb_prefetch_adjacent_diff(const float *points, uint32_t num_points,
  * (src/aabb_tree/aabb_tree.h:18-27) for the one use the tracer has for it: the start cell of a camera
  * (radfoam_model/scene.py:224-234).  A tiled brute force: U x N distance evaluations, 12 N bytes of traffic in
  * total; meant for camera counts (1 .. a few thousand queries).  points[N][3], queries[M][3] f32, indices[M]
- * u32, all device pointers. */
+ * u32, all device pointers.  For many distinct queries rfb_locate_points is the scalable lookup. */
 int rfb_nearest_point(const float *points, uint32_t num_points, const float *queries,
                       uint32_t num_queries, uint32_t *indices, void *stream);
 
@@ -173,6 +175,51 @@ int rfb_farthest_neighbor(const float *points, uint32_t num_points,
                           const uint32_t *point_adjacency,
                           const uint32_t *point_adjacency_offsets,
                           uint32_t *indices, float *cell_radius, void *stream);
+
+/* Cell of any number of query points, found by walking the adjacency graph (radfoam::nn over the AABB tree,
+ * src/aabb_tree/aabb_tree.cu:343-415, answers the same question).  From a seed cell s the walk scans row s of the
+ * CSR and moves to the neighbour smallest in the order (d2, index) -- d2 = fma(dx,dx, fma(dy,dy, dz*dz)) in fp32,
+ * as rfb_nearest_point computes it, ties to the lower index -- and stops when no neighbour is smaller than s.
+ * Seeds: hints[m] when it is < num_points; when it is not, or hints is NULL, the library's seed (the nearest of a
+ * fixed strided sample of the points).  Cost: the walk's row scans (about 15.5 distances each) per query, instead
+ * of rfb_nearest_point's N.  Contract:
+ *   - indices[m] is always a local minimum of (d2, index) over the adjacency graph (empty rows are legal: the
+ *     walk stops there);
+ *   - when the adjacency is the Delaunay graph of `points`, it is the nearest point as rfb_nearest_point defines
+ *     it, except for queries whose best and second-best distances are within fp32 rounding of each other;
+ *   - when the points have moved since the adjacency was built (a stale triangulation) only the local-minimum
+ *     property holds (a stale AABB tree promises no more);
+ *   - a query with a NaN coordinate, or whose cell is at a non-finite distance, yields UINT32_MAX.
+ * No host synchronisation, no allocation; safe under CUDA-graph capture.  points[N][3], queries[M][3] f32,
+ * CSR as for the tracer, hints[M] / indices[M] u32, all device pointers. */
+int rfb_locate_points(const float *points, uint32_t num_points,
+                      const uint32_t *point_adjacency, const uint32_t *point_adjacency_offsets,
+                      const float *queries, uint32_t num_queries,
+                      const uint32_t *hints, uint32_t *indices, void *stream);
+
+/* The field at M query points: cells[m] = rfb_locate_points' cell (same seeds, same contract),
+ * density[m] = attributes[cell][A-1] and, when directions[M][3] is given (renormalised in the kernel, as ray
+ * directions are), rgb[m][3] = max(0, 0.5 + sum_k Y_k(dir) c_k): the colour the tracer composites for that cell
+ * along a ray with that direction, bit for bit (same SH basis and FFMA chain).  directions and rgb are both given
+ * or both NULL.  density and rgb are in the pipeline's attribute dtype; a query without a cell (UINT32_MAX) gets
+ * NaN.  Reads only its arguments: no pipeline state (scene mirrors, walk tape, accumulator) is used or changed. */
+int rfb_sample_field(rfb_pipeline *pipeline, const float *points, uint32_t num_points, const void *attributes,
+                     const uint32_t *point_adjacency, const uint32_t *point_adjacency_offsets,
+                     const float *queries, uint32_t num_queries, const uint32_t *hints,
+                     const float *directions, uint32_t *cells, void *density, void *rgb, void *stream);
+
+/* Backward of rfb_sample_field with respect to the attributes: attribute_grad[N][A] (attr dtype) is fully
+ * overwritten with sum over queries m in cell i of  Y_k(dir_m) dL/drgb_m[c]  at column 3k+c (0 where the forward's
+ * rgb_m[c] is 0, the clamp) and dL/ddensity_m at column A-1.  Summed in fp32, rounded once to the attribute dtype.
+ * rgb_grad[M][3] / density_grad[M] (attr dtype) may each be NULL (no gradient); rgb_grad needs directions and the
+ * forward's rgb.  Queries whose cell is not a point (UINT32_MAX) contribute nothing.  The gradients with respect to
+ * points and queries are zero almost everywhere (the field is piecewise constant) and are not formed; those with
+ * respect to the directions are not computed.  Uses stream-ordered scratch for fp16, never the pipeline's
+ * accumulator: a recorded walk tape or accumulated trace gradients stay as they were. */
+int rfb_sample_field_backward(rfb_pipeline *pipeline, uint32_t num_points, uint32_t num_queries,
+                              const uint32_t *cells, const float *directions, const void *rgb,
+                              const void *rgb_grad, const void *density_grad, void *attribute_grad,
+                              void *stream);
 
 int rfb_trace_forward(rfb_pipeline *pipeline, const rfb_trace_settings *settings,
                       uint32_t num_points, const float *points,

@@ -13,15 +13,16 @@ no CPU fallback).
 """
 from . import foam  # noqa: F401  (numpy/scipy only)
 
-__all__ = ["create_pipeline", "Pipeline", "TraceRays", "TraceRaysParams", "ShardedTracer", "nearest_point", "starting_points",
-           "farthest_neighbor", "foam", "library_path"]
+__all__ = ["create_pipeline", "Pipeline", "TraceRays", "TraceRaysParams", "SampleField", "ShardedTracer",
+           "nearest_point", "starting_points", "locate_points", "farthest_neighbor", "foam", "library_path"]
 
 
 def __getattr__(name):
-    if name in ("create_pipeline", "Pipeline", "nearest_point", "starting_points", "farthest_neighbor"):
+    if name in ("create_pipeline", "Pipeline", "nearest_point", "starting_points", "locate_points",
+                "farthest_neighbor"):
         from . import pipeline as _p
         return getattr(_p, name)
-    if name in ("TraceRays", "TraceRaysParams"):
+    if name in ("TraceRays", "TraceRaysParams", "SampleField"):
         from . import render as _r
         return getattr(_r, name)
     if name == "ShardedTracer":

@@ -70,6 +70,9 @@ SIGNATURES = {
     "rfb_nearest_point": (c_int, [_P, c_uint32, _P, c_uint32, _P, _P]),
     "rfb_start_points": (c_int, [_P, c_uint32, _P, c_uint32, _P, _P]),
     "rfb_farthest_neighbor": (c_int, [_P, c_uint32, _P, _P, _P, _P, _P]),
+    "rfb_locate_points": (c_int, [_P, c_uint32, _P, _P, _P, c_uint32, _P, _P, _P]),
+    "rfb_sample_field": (c_int, [_P, _P, c_uint32, _P, _P, _P, _P, c_uint32, _P, _P, _P, _P, _P, _P]),
+    "rfb_sample_field_backward": (c_int, [_P, c_uint32, c_uint32, _P, _P, _P, _P, _P, _P, _P]),
     "rfb_trace_forward": (c_int, [_P, POINTER(TraceSettings), c_uint32, _P, _P, c_uint32, _P, _P,
                                   c_uint32, _P, _P, c_uint32, _P, _P, _P, _P, _P, _P,
                                   POINTER(LaunchOpts), _P]),

@@ -180,8 +180,22 @@ __device__ __forceinline__ void sh_basis(float x, float y, float z, float *sh) {
 }
 
 // rgb = max(0, 0.5 + sum_k Y_k * c_k) per channel, accumulated k ascending in one
-// FFMA chain per channel (load_sh_as_rgb, sh_utils.cuh:72-83).  `row` is the
-// 16-byte aligned internal SH row [3*sh_dim floats, channel-interleaved][pad].
+// FFMA chain per channel (load_sh_as_rgb, sh_utils.cuh:72-83), from the 3*sh_dim
+// channel-interleaved coefficients `v`.
+template <int DEG>
+__device__ __forceinline__ void sh_coeffs_to_rgb(const float *v, const float *sh, float &r, float &g, float &b) {
+    float rgb[3] = {0.5f, 0.5f, 0.5f};
+#pragma unroll
+    for (int i = 0; i < 3 * sh_dim(DEG); ++i)
+        rgb[i % 3] = __fmaf_rn(sh[i / 3], v[i], rgb[i % 3]);
+    // cwiseMax(0): (x < 0) ? 0 : x  (NaN stays NaN, as in the reference build)
+    r = (rgb[0] < 0.0f) ? 0.0f : rgb[0];
+    g = (rgb[1] < 0.0f) ? 0.0f : rgb[1];
+    b = (rgb[2] < 0.0f) ? 0.0f : rgb[2];
+}
+
+// sh_coeffs_to_rgb of one row of the internal SH mirror: `row` is 16-byte aligned
+// [3*sh_dim floats, channel-interleaved][pad].
 template <int DEG>
 __device__ __forceinline__ void sh_to_rgb(const float *__restrict__ row, const float *sh,
                                           float &r, float &g, float &b) {
@@ -196,14 +210,7 @@ __device__ __forceinline__ void sh_to_rgb(const float *__restrict__ row, const f
         v[4 * i + 2] = q.z;
         v[4 * i + 3] = q.w;
     }
-    float rgb[3] = {0.5f, 0.5f, 0.5f};
-#pragma unroll
-    for (int i = 0; i < 3 * sh_dim(DEG); ++i)
-        rgb[i % 3] = __fmaf_rn(sh[i / 3], v[i], rgb[i % 3]);
-    // cwiseMax(0): (x < 0) ? 0 : x  (NaN stays NaN, as in the reference build)
-    r = (rgb[0] < 0.0f) ? 0.0f : rgb[0];
-    g = (rgb[1] < 0.0f) ? 0.0f : rgb[1];
-    b = (rgb[2] < 0.0f) ? 0.0f : rgb[2];
+    sh_coeffs_to_rgb<DEG>(v, sh, r, g, b);
 }
 
 // ---------------------------------------------------------------- the walk

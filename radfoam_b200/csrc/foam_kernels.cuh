@@ -1363,6 +1363,233 @@ __global__ void start_points_scatter_kernel(const uint32_t *__restrict__ slot_of
         start[r] = (uint32_t)best[query_of_slot[slot_of_ray[r]]];
 }
 
+// ------------------------------------------------------------------ point location by walking the adjacency graph
+// The CSR adjacency the tracer takes is the Delaunay graph of the points, and on a Delaunay graph a greedy walk
+// reaches the nearest site: when s is not the nearest point of q, the segment s -> q leaves the Voronoi cell of s
+// through a face shared with a Delaunay neighbour j, and beyond that face j is strictly closer to q than s.  So
+// every query costs a handful of row scans (about 15.5 distances each) from a nearby seed, with no tree to build
+// or keep current while the points move.
+//   Order: (d2, index) packed into one 64-bit key -- distance bits above the index, exactly "smaller distance,
+//   lower index among equals" (rfb_nearest_point's rule); NaN distances count as +inf.  d2 in the x0 + (x1 + x2)
+//   fma order of nearest_points_kernel.  A step moves to the smallest key of the row and is taken only if that
+//   key is smaller than the current one, so the walk terminates on any adjacency (the key strictly decreases).
+//   Seed: the hint when it names a point, else the nearest of a fixed strided sample of the points (spatially
+//   sorted points make a strided sample an even cover of the scene; unsorted points only make the walks longer).
+//   The sample streams through shared memory in tiles, every thread of the CTA reading the same entry.
+constexpr uint32_t kLocateTile = 1024;
+
+struct LocateParams {
+    const float *points;
+    const uint32_t *adj, *off;
+    const float *queries;
+    const uint32_t *hints; // nullptr: every seed from the sample
+    uint32_t num_points, num_queries;
+    uint32_t sample, stride; // seed sample: points[k * stride], k < sample
+};
+
+__device__ __forceinline__ float query_d2(float px, float py, float pz, float qx, float qy, float qz) {
+    const float dx = __fsub_rn(px, qx), dy = __fsub_rn(py, qy), dz = __fsub_rn(pz, qz);
+    return __fmaf_rn(dx, dx, __fmaf_rn(dy, dy, __fmul_rn(dz, dz)));
+}
+
+__device__ __forceinline__ unsigned long long locate_key(float d2, uint32_t i) {
+    const uint32_t bits = d2 != d2 ? 0x7f800000u : __float_as_uint(d2); // d2 >= +0: the bits order like the floats
+    return ((unsigned long long)bits << 32) | i;
+}
+
+__device__ __forceinline__ unsigned long long point_key(const float *__restrict__ points, uint32_t j, float qx,
+                                                        float qy, float qz) {
+    const uint64_t b = 3 * (uint64_t)j;
+    return locate_key(query_d2(__ldg(points + b), __ldg(points + b + 1), __ldg(points + b + 2), qx, qy, qz), j);
+}
+
+// The greedy walk from `s`: the key of the local minimum it ends in.
+__device__ __forceinline__ unsigned long long walk_to_nearest(const LocateParams &p, uint32_t s, float qx, float qy,
+                                                              float qz) {
+    unsigned long long key = point_key(p.points, s, qx, qy, qz);
+    for (;;) {
+        unsigned long long best = key;
+        const uint32_t end = __ldg(p.off + s + 1);
+        for (uint32_t e = __ldg(p.off + s); e < end; ++e) {
+            const unsigned long long k = point_key(p.points, __ldg(p.adj + e), qx, qy, qz);
+            best = k < best ? k : best;
+        }
+        if (best == key)
+            return key;
+        key = best;
+        s = (uint32_t)best;
+    }
+}
+
+// Cell of query q: UINT32_MAX for q >= num_queries, for a NaN coordinate, and when even the cell found is at a
+// non-finite distance (rfb_nearest_point finds no point then either).  Every thread of the CTA must call it: the
+// seed search synchronises.
+__device__ __forceinline__ uint32_t locate_point(const LocateParams &p, uint32_t q) {
+    __shared__ float4 tile[kLocateTile];
+    __shared__ int seeds_wanted;
+    const bool live = q < p.num_queries;
+    float qx = 0.0f, qy = 0.0f, qz = 0.0f;
+    uint32_t seed = kNone;
+    if (live) {
+        qx = __ldg(p.queries + 3 * (uint64_t)q);
+        qy = __ldg(p.queries + 3 * (uint64_t)q + 1);
+        qz = __ldg(p.queries + 3 * (uint64_t)q + 2);
+        if (p.hints) {
+            const uint32_t h = __ldg(p.hints + q);
+            seed = h < p.num_points ? h : kNone;
+        }
+    }
+    const bool nan = qx != qx || qy != qy || qz != qz;
+    const bool need = live && !nan && seed == kNone;
+    if (threadIdx.x == 0)
+        seeds_wanted = 0;
+    __syncthreads();
+    if (need)
+        seeds_wanted = 1;
+    __syncthreads();
+    if (seeds_wanted) {
+        float best_d = __int_as_float(0x7f800000);
+        uint32_t best_i = 0; // no sample point at a finite distance: start from point 0
+        for (uint32_t t0 = 0; t0 < p.sample; t0 += kLocateTile) {
+            const uint32_t cnt = p.sample - t0 < kLocateTile ? p.sample - t0 : kLocateTile;
+            __syncthreads();
+            for (uint32_t i = threadIdx.x; i < cnt; i += blockDim.x) {
+                const uint64_t j = 3 * ((uint64_t)(t0 + i) * p.stride);
+                tile[i] = make_float4(__ldg(p.points + j), __ldg(p.points + j + 1), __ldg(p.points + j + 2), 0.0f);
+            }
+            __syncthreads();
+            if (need)
+                for (uint32_t i = 0; i < cnt; ++i) {
+                    const float4 pt = tile[i];
+                    const float d2 = query_d2(pt.x, pt.y, pt.z, qx, qy, qz);
+                    if (d2 < best_d) { // strict, indices ascending: the lowest index among equals stays
+                        best_d = d2;
+                        best_i = (t0 + i) * p.stride;
+                    }
+                }
+        }
+        if (need)
+            seed = best_i;
+    }
+    if (!live || nan)
+        return kNone;
+    const unsigned long long key = walk_to_nearest(p, seed, qx, qy, qz);
+    return (key >> 32) >= 0x7f800000ull ? kNone : (uint32_t)key;
+}
+
+__global__ void __launch_bounds__(256) locate_points_kernel(const LocateParams p, uint32_t *__restrict__ indices) {
+    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t cell = locate_point(p, q);
+    if (q < p.num_queries)
+        indices[q] = cell;
+}
+
+// ------------------------------------------------------------------ field sampling
+// The field at a point is its cell's attribute row: density = the last column, and the colour seen along a unit
+// direction d = max(0, 0.5 + sum_k Y_k(d) c_k) with the tracer's own basis and FFMA chain (sh_basis,
+// sh_coeffs_to_rgb), read from the caller's attributes -- the same floats the tracer's SH mirror holds -- so that
+// it is the colour the tracer composites for that cell along a ray with direction d.  A query without a cell
+// (UINT32_MAX) gets NaN.
+template <int DEG, typename AttrT>
+__global__ void __launch_bounds__(256) sample_field_kernel(const LocateParams p, const AttrT *__restrict__ attrs,
+                                                           const float *__restrict__ dirs,
+                                                           uint32_t *__restrict__ cells, AttrT *__restrict__ density,
+                                                           AttrT *__restrict__ rgb) {
+    constexpr int A = attr_dim(DEG), NC = 3 * sh_dim(DEG);
+    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t cell = locate_point(p, q);
+    if (q >= p.num_queries)
+        return;
+    cells[q] = cell;
+    const float nan = __int_as_float(0x7fc00000);
+    if (cell == kNone) {
+        density[q] = (AttrT)nan;
+        if (rgb)
+            rgb[3 * (uint64_t)q] = rgb[3 * (uint64_t)q + 1] = rgb[3 * (uint64_t)q + 2] = (AttrT)nan;
+        return;
+    }
+    const AttrT *row = attrs + (uint64_t)cell * A;
+    density[q] = row[A - 1];
+    if (!rgb)
+        return;
+    float dx = __ldg(dirs + 3 * (uint64_t)q), dy = __ldg(dirs + 3 * (uint64_t)q + 1),
+          dz = __ldg(dirs + 3 * (uint64_t)q + 2);
+    normalize_dir(dx, dy, dz);
+    float sh[sh_dim(DEG)];
+    sh_basis<DEG>(dx, dy, dz, sh);
+    float v[NC];
+#pragma unroll
+    for (int i = 0; i < NC; ++i)
+        v[i] = (float)row[i];
+    float r, g, b;
+    sh_coeffs_to_rgb<DEG>(v, sh, r, g, b);
+    rgb[3 * (uint64_t)q] = (AttrT)r;
+    rgb[3 * (uint64_t)q + 1] = (AttrT)g;
+    rgb[3 * (uint64_t)q + 2] = (AttrT)b;
+}
+
+// Backward of the sampling: acc[cell][3k + c] += Y_k(d) * dL/drgb_c (0 where the forward's rgb_c is 0, the
+// tracer's ReLU mask) and acc[cell][A - 1] += dL/ddensity, in fp32.  Grid sampling puts many queries in one cell,
+// so a warp first sums the rows of its lanes that share a cell: every lane stages its row in shared memory, the
+// lanes of a group split the columns between them, and each column of a group reaches L2 as ONE atomic.
+constexpr int kSampleBwdBlock = 128;
+
+template <int DEG, typename AttrT>
+__global__ void __launch_bounds__(kSampleBwdBlock) sample_field_backward_kernel(
+    const uint32_t *__restrict__ cells, uint32_t num_queries, uint32_t num_points, const float *__restrict__ dirs,
+    const AttrT *__restrict__ rgb, const AttrT *__restrict__ rgb_grad, const AttrT *__restrict__ density_grad,
+    float *__restrict__ acc) {
+    constexpr int A = attr_dim(DEG), NC = 3 * sh_dim(DEG);
+    __shared__ float rows[kSampleBwdBlock / 32][32][A];
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t cell = q < num_queries ? __ldg(cells + q) : kNone;
+    if (cell >= num_points)
+        cell = kNone; // a query that found no cell has no gradient
+    if (cell != kNone) {
+        float *row = rows[warp][lane];
+        if (rgb_grad) {
+            float dx = __ldg(dirs + 3 * (uint64_t)q), dy = __ldg(dirs + 3 * (uint64_t)q + 1),
+                  dz = __ldg(dirs + 3 * (uint64_t)q + 2);
+            normalize_dir(dx, dy, dz);
+            float sh[sh_dim(DEG)];
+            sh_basis<DEG>(dx, dy, dz, sh);
+            float g[3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c)
+                g[c] = (float)rgb[3 * (uint64_t)q + c] == 0.0f ? 0.0f : (float)rgb_grad[3 * (uint64_t)q + c];
+#pragma unroll
+            for (int i = 0; i < NC; ++i)
+                row[i] = __fmul_rn(sh[i / 3], g[i % 3]);
+        } else {
+#pragma unroll
+            for (int i = 0; i < NC; ++i)
+                row[i] = 0.0f;
+        }
+        row[A - 1] = density_grad ? (float)density_grad[q] : 0.0f;
+    }
+    const unsigned peers = __match_any_sync(0xffffffffu, cell);
+    __syncwarp();
+    if (cell == kNone)
+        return;
+    const int size = __popc(peers), rank = __popc(peers & ((1u << lane) - 1u));
+    for (int c = rank; c < A; c += size) {
+        float s = 0.0f;
+        for (unsigned m = peers; m; m &= m - 1u)
+            s = __fadd_rn(s, rows[warp][__ffs(m) - 1][c]);
+        if (s != 0.0f)
+            atomicAdd(acc + (uint64_t)cell * A + c, s);
+    }
+}
+
+// attribute_grad = the fp32 accumulator rounded once to the attribute dtype
+__global__ void __launch_bounds__(256) round_to_half_kernel(const float *__restrict__ acc, uint64_t n,
+                                                            __half *__restrict__ out) {
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+        out[i] = __float2half_rn(acc[i]);
+}
+
 // ------------------------------------------------------------------ farthest neighbour (SURVEY.md §8f.4)
 // Per cell: the adjacent point farthest from it and half the mean neighbour distance ("cell radius"),
 // what the densification pass reads (scene.py:434-461; reference kernel triangulation_ops.cu:9-44).

@@ -892,6 +892,126 @@ int rfb_farthest_neighbor(const float *points, uint32_t num_points, const uint32
     return 0;
 }
 
+} // extern "C"
+
+namespace {
+// Points in the seed sample of rfb_locate_points (DESIGN.md §4: the measured trade-off between the sample scan every
+// query pays and the walk it shortens).  RFB_LOCATE_SAMPLE overrides it per call, for measuring that trade-off and
+// for tests that want long walks on small foams; on a Delaunay adjacency the results do not depend on it (up to
+// fp32 near-ties).
+constexpr uint32_t kLocateSample = 2048;
+
+LocateParams locate_params(const float *points, uint32_t num_points, const uint32_t *adj, const uint32_t *off,
+                           const float *queries, uint32_t num_queries, const uint32_t *hints) {
+    const char *e = getenv("RFB_LOCATE_SAMPLE");
+    const long v = e ? atol(e) : 0;
+    const uint32_t sample = v > 0 && v < (1l << 30) ? (uint32_t)v : kLocateSample;
+    LocateParams lp;
+    lp.points = points;
+    lp.adj = adj;
+    lp.off = off;
+    lp.queries = queries;
+    lp.hints = hints;
+    lp.num_points = num_points;
+    lp.num_queries = num_queries;
+    lp.sample = sample < num_points ? sample : num_points;
+    lp.stride = num_points / lp.sample;
+    return lp;
+}
+} // namespace
+
+extern "C" {
+
+int rfb_locate_points(const float *points, uint32_t num_points, const uint32_t *point_adjacency,
+                      const uint32_t *point_adjacency_offsets, const float *queries, uint32_t num_queries,
+                      const uint32_t *hints, uint32_t *indices, void *stream) {
+    if (num_queries == 0)
+        return 0;
+    // point_adjacency may be NULL only when every row is empty; the kernel never reads it then
+    if (!points || !point_adjacency_offsets || !queries || !indices)
+        return fail("rfb_locate_points: NULL argument");
+    if (num_points == 0)
+        return fail("rfb_locate_points: empty point set");
+    const LocateParams lp = locate_params(points, num_points, point_adjacency, point_adjacency_offsets, queries,
+                                          num_queries, hints);
+    RFB_LAUNCH((rfb::locate_points_kernel), (num_queries + 255) / 256, 256, 0, (cudaStream_t)stream, lp, indices);
+    RFB_LAUNCHED();
+    return 0;
+}
+
+int rfb_sample_field(rfb_pipeline *p, const float *points, uint32_t num_points, const void *attributes,
+                     const uint32_t *point_adjacency, const uint32_t *point_adjacency_offsets, const float *queries,
+                     uint32_t num_queries, const uint32_t *hints, const float *directions, uint32_t *cells,
+                     void *density, void *rgb, void *stream) {
+    if (!p)
+        return fail("rfb_sample_field: pipeline is NULL");
+    if ((directions == nullptr) != (rgb == nullptr))
+        return fail("rfb_sample_field: directions and rgb must both be given or both be NULL");
+    if (num_queries == 0)
+        return 0;
+    if (!points || !attributes || !point_adjacency_offsets || !queries || !cells || !density)
+        return fail("rfb_sample_field: NULL argument");
+    if (num_points == 0)
+        return fail("rfb_sample_field: empty point set");
+    const LocateParams lp = locate_params(points, num_points, point_adjacency, point_adjacency_offsets, queries,
+                                          num_queries, hints);
+    with_degree(p->sh_degree, [&](auto d) {
+        with_attr_type(p->attr_dtype, [&](auto t) {
+            using AttrT = typename decltype(t)::type;
+            RFB_LAUNCH((sample_field_kernel<decltype(d)::value, AttrT>), (num_queries + 255) / 256, 256, 0,
+                       (cudaStream_t)stream, lp, reinterpret_cast<const AttrT *>(attributes), directions, cells,
+                       reinterpret_cast<AttrT *>(density), reinterpret_cast<AttrT *>(rgb));
+        });
+    });
+    RFB_LAUNCHED();
+    return 0;
+}
+
+int rfb_sample_field_backward(rfb_pipeline *p, uint32_t num_points, uint32_t num_queries, const uint32_t *cells,
+                              const float *directions, const void *rgb, const void *rgb_grad,
+                              const void *density_grad, void *attribute_grad, void *stream_) {
+    if (!p)
+        return fail("rfb_sample_field_backward: pipeline is NULL");
+    if (rgb_grad && (!directions || !rgb))
+        return fail("rfb_sample_field_backward: rgb_grad needs the directions and the forward's rgb");
+    if (num_points == 0)
+        return 0;
+    if (!attribute_grad || (num_queries && !cells))
+        return fail("rfb_sample_field_backward: NULL argument");
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const uint64_t entries = (uint64_t)num_points * attr_dim(p->sh_degree);
+    const bool half = p->attr_dtype == RFB_FLOAT16;
+    // fp32 attributes: accumulate in place; fp16: in stream-ordered fp32 scratch, rounded once at the end
+    float *acc = reinterpret_cast<float *>(attribute_grad);
+    if (half)
+        if (int rc = stream_scratch(reinterpret_cast<void **>(&acc), entries * sizeof(float), stream))
+            return rc;
+    cudaMemsetAsync(acc, 0, entries * sizeof(float), stream);
+    if (num_queries) {
+        with_degree(p->sh_degree, [&](auto d) {
+            with_attr_type(p->attr_dtype, [&](auto t) {
+                using AttrT = typename decltype(t)::type;
+                RFB_LAUNCH((sample_field_backward_kernel<decltype(d)::value, AttrT>),
+                           (num_queries + kSampleBwdBlock - 1) / kSampleBwdBlock, kSampleBwdBlock, 0, stream, cells,
+                           num_queries, num_points, directions, reinterpret_cast<const AttrT *>(rgb),
+                           reinterpret_cast<const AttrT *>(rgb_grad), reinterpret_cast<const AttrT *>(density_grad),
+                           acc);
+            });
+        });
+        ++g_launches;
+    }
+    if (half) {
+        RFB_LAUNCH((round_to_half_kernel), grid_for(entries, 256), 256, 0, stream, (const float *)acc, entries,
+                   reinterpret_cast<__half *>(attribute_grad));
+        ++g_launches;
+    }
+    const cudaError_t launched = cudaGetLastError();
+    if (half)
+        cudaFreeAsync(acc, stream); // stream-ordered: after the kernels above, also on the error path
+    RFB_CUDA(launched);
+    return 0;
+}
+
 int rfb_trace_forward(rfb_pipeline *p, const rfb_trace_settings *settings, uint32_t num_points,
                       const float *points, const void *attributes, uint32_t point_adjacency_size,
                       const uint32_t *point_adjacency, const uint32_t *point_adjacency_offsets,

@@ -791,6 +791,75 @@ class Pipeline:
                 _ptr(output_rgba), ctypes.byref(opts), stream))
         return output_rgba.view(cam.height, cam.width)
 
+    # ---- the field at arbitrary points (rfb_sample_field): not part of the reference's Pipeline
+    def sample_field(self, points, attributes, point_adjacency, point_adjacency_offsets, queries, directions=None,
+                     hint=None):
+        """The field at query points ``[..., 3]``: ``{"cell": uint32[...], "density": [...], "rgb": [..., 3]}`` --
+        the cell of each query (as :func:`locate_points` finds it, ``hint`` likewise), its density (the attribute
+        row's last column) and, when ``directions [..., 3]`` are given, the colour the tracer composites for that
+        cell along a ray with that direction.  density and rgb are in the pipeline's attribute dtype; a query
+        without a cell (a NaN coordinate) gets NaN.  Differentiable with respect to ``attributes`` through
+        :class:`radfoam_b200.SampleField`."""
+        self._validate_scene(points, attributes, point_adjacency, point_adjacency_offsets)
+        if attributes is None:
+            raise RuntimeError("sample_field needs the attributes (a bound parameter-form scene is not used here)")
+        pts, attrs = points.detach().contiguous(), attributes.detach().contiguous()
+        adj, off = point_adjacency.contiguous(), point_adjacency_offsets.contiguous()
+        q, batch = _query_points(queries, pts.device)
+        hints = _hints(hint, batch, pts.device)
+        d = None
+        if directions is not None:
+            d = directions.detach()
+            if d.dtype != torch.float32 or d.device != pts.device or tuple(d.shape) != batch + (3,):
+                raise RuntimeError("directions must be float32 [..., 3] on the queries' device, one per query")
+            d = d.contiguous()
+        m = q.size(0)
+        cell = torch.empty(batch, dtype=torch.uint32, device=pts.device)
+        density = torch.empty(batch, dtype=self._dtype, device=pts.device)
+        rgb = torch.empty(batch + (3,), dtype=self._dtype, device=pts.device) if d is not None else None
+        with torch.cuda.device(pts.device):
+            stream = torch.cuda.current_stream(pts.device).cuda_stream
+            _lib.check(self._lib.rfb_sample_field(
+                self._handle, _ptr(pts), pts.size(0), _ptr(attrs), _ptr(adj) if adj.numel() else None, _ptr(off),
+                _ptr(q), m, _ptr(hints), _ptr(d), _ptr(cell), _ptr(density), _ptr(rgb), stream))
+        out = {"cell": cell, "density": density}
+        if rgb is not None:
+            out["rgb"] = rgb
+        return out
+
+    def sample_field_backward(self, num_points, cell, directions=None, rgb=None, rgb_grad=None, density_grad=None):
+        """Gradient of a :meth:`sample_field` call's outputs with respect to the attributes: ``[num_points, A]`` in
+        the attribute dtype, summed in fp32 over the queries of each cell and rounded once.  ``rgb`` is the forward's
+        colour output (its zeros mask the clamp); ``rgb_grad`` needs ``directions`` and ``rgb``.  The pipeline's
+        own state (scene mirrors, walk tape, gradient accumulator) is not touched."""
+        c = cell.detach().contiguous()
+        if c.dtype != torch.uint32 or c.device.type != "cuda":
+            raise RuntimeError("cell must be the uint32 CUDA tensor sample_field returned")
+        batch, m = tuple(c.shape), c.numel()
+
+        def per_query(name, t, cols, dtype):
+            if t is None:
+                return None
+            t = t.detach()
+            if t.dtype != dtype or t.device != c.device or tuple(t.shape) != batch + cols:
+                raise RuntimeError(f"{name} must be {_dtype_name(dtype)} with shape {list(batch + cols)} "
+                                   "on the cell's device")
+            return t.contiguous()
+
+        d = per_query("directions", directions, (3,), torch.float32)
+        rgb_c = per_query("rgb", rgb, (3,), self._dtype)
+        g_c = per_query("rgb_grad", rgb_grad, (3,), self._dtype)
+        dg_c = per_query("density_grad", density_grad, (), self._dtype)
+        if g_c is not None and (d is None or rgb_c is None):
+            raise RuntimeError("rgb_grad needs the directions and the forward's rgb")
+        attr_grad = torch.empty((int(num_points), self._attr_dim), dtype=self._dtype, device=c.device)
+        with torch.cuda.device(c.device):
+            stream = torch.cuda.current_stream(c.device).cuda_stream
+            _lib.check(self._lib.rfb_sample_field_backward(
+                self._handle, int(num_points), m, _ptr(c), _ptr(d), _ptr(rgb_c), _ptr(g_c), _ptr(dg_c),
+                _ptr(attr_grad), stream))
+        return attr_grad
+
     # radfoam::prefetch_adjacent_diff (pipeline.h:50-56); handy for trace_benchmark callers
     def prefetch_adjacent_diff(self, points, point_adjacency, point_adjacency_offsets):
         points_c = points.contiguous()
@@ -856,6 +925,84 @@ def starting_points(rays, points):
     with torch.cuda.device(pts.device):
         stream = torch.cuda.current_stream(pts.device).cuda_stream
         _lib.check(_lib.load().rfb_start_points(_ptr(pts), pts.size(0), _ptr(r), r.numel() // 6, _ptr(out), stream))
+    return out
+
+
+def _query_points(queries, device):
+    """(contiguous float32 [M, 3] view, batch shape) of query points [..., 3]."""
+    if queries.dtype != torch.float32 or queries.size(-1) != 3:
+        raise RuntimeError("queries must be float32 [..., 3]")
+    if queries.device != device:
+        raise RuntimeError("queries must be on the same CUDA device as points")
+    return queries.detach().contiguous().view(-1, 3), tuple(queries.shape[:-1])
+
+
+def _hints(hint, batch, device):
+    """uint32 [M] start cells of the walk from ``hint``: None, an int (one cell for every query) or a uint32 / int
+    tensor of the queries' batch shape.  Values >= num_points leave the seed to the library."""
+    if hint is None:
+        return None
+    if not isinstance(hint, torch.Tensor):
+        h = int(hint)
+        if h < 0:
+            raise RuntimeError("hint must be a non-negative cell index")
+        h = min(h, 0xFFFFFFFF)
+        m = 1
+        for s in batch:
+            m *= s
+        return torch.full((m,), h, dtype=torch.int64, device=device).to(torch.uint32)
+    if tuple(hint.shape) != batch:
+        raise RuntimeError(f"hint must have the queries' batch shape {list(batch)}")
+    if hint.device != device:
+        raise RuntimeError("hint must be on the same CUDA device as points")
+    if hint.dtype == torch.uint32:
+        return hint.detach().contiguous().view(-1)
+    if hint.dtype in (torch.int32, torch.int64):
+        return hint.detach().reshape(-1).clamp(0, 0xFFFFFFFF).to(torch.int64).to(torch.uint32)
+    raise RuntimeError("hint must be an integer tensor (uint32, int32 or int64)")
+
+
+def _csr(points, point_adjacency, point_adjacency_offsets):
+    """Validated contiguous (points [N, 3], adjacency, offsets) of a foam, as farthest_neighbor takes them."""
+    if points.device.type != "cuda":
+        raise RuntimeError("points must be on CUDA device")
+    pts = points.detach().contiguous()
+    if pts.dtype != torch.float32:
+        raise RuntimeError("points must have float32 dtype")
+    if pts.dim() != 2 or pts.size(-1) != 3:
+        raise RuntimeError("points must have shape [N, 3]")
+    adj = point_adjacency.detach().contiguous()
+    off = point_adjacency_offsets.detach().contiguous()
+    for name, t in (("point_adjacency", adj), ("point_adjacency_offsets", off)):
+        if t.dtype != torch.uint32:
+            raise RuntimeError(f"{name} must have uint32 dtype")
+        if t.device != pts.device:
+            raise RuntimeError(f"{name} must be on the same device as points")
+    if off.numel() != pts.size(0) + 1:
+        raise RuntimeError("point_adjacency_offsets must have num_points + 1 elements")
+    return pts, adj, off
+
+
+def locate_points(points, point_adjacency, point_adjacency_offsets, queries, hint=None):
+    """Cell of every query point ``[..., 3]`` (``uint32`` in the queries' batch shape) by a greedy walk over the
+    adjacency graph: the nearest point, as :func:`nearest_point` defines it, when the adjacency is the Delaunay
+    graph of ``points`` (up to fp32 near-ties); a local minimum of the distance over the graph when the points have
+    moved since it was built.  ``hint``: a start cell per query (e.g. the ``depth_indices`` of the ray that reached
+    it) or one int for all; a hint that is not a cell, or none, lets the library seed the walk.  A query with a NaN
+    coordinate gets UINT32_MAX.  Costs a few row scans per query -- use it for many distinct queries, where
+    :func:`nearest_point` costs N distances each."""
+    pts, adj, off = _csr(points, point_adjacency, point_adjacency_offsets)
+    q, batch = _query_points(queries, pts.device)
+    hints = _hints(hint, batch, pts.device)
+    out = torch.empty(batch, dtype=torch.uint32, device=pts.device)
+    if q.size(0) == 0:
+        return out
+    if pts.size(0) == 0:
+        raise RuntimeError("locate_points: empty point set")
+    with torch.cuda.device(pts.device):
+        stream = torch.cuda.current_stream(pts.device).cuda_stream
+        _lib.check(_lib.load().rfb_locate_points(_ptr(pts), pts.size(0), _ptr(adj) if adj.numel() else None,
+                                                 _ptr(off), _ptr(q), q.size(0), _ptr(hints), _ptr(out), stream))
     return out
 
 

@@ -80,6 +80,40 @@ class TraceRays(torch.autograd.Function):
                  grads["ray_grad"] if want_rays else None) + (None,) * 3)
 
 
+class SampleField(torch.autograd.Function):
+    """The field at query points, differentiable with respect to the attributes:
+    ``SampleField.apply(pipeline, points, attributes, point_adjacency, point_adjacency_offsets, queries, directions,
+    hint)`` -> ``(density [...], rgb [..., 3] or None, cell uint32 [...])`` (see ``Pipeline.sample_field``).  The
+    field is piecewise constant in space, so the gradient with respect to ``points`` is zero almost everywhere
+    (returned as None); gradients with respect to ``queries`` and ``directions`` are not computed, and asking for
+    them is an error."""
+
+    @staticmethod
+    def forward(ctx, pipeline, points, attributes, point_adjacency, point_adjacency_offsets, queries,
+                directions=None, hint=None):
+        for name, t in (("queries", queries), ("directions", directions)):
+            if t is not None and t.requires_grad:
+                raise RuntimeError(f"SampleField: gradients with respect to {name} are not computed; pass "
+                                   f"{name}.detach()")
+        out = pipeline.sample_field(points, attributes, point_adjacency, point_adjacency_offsets, queries,
+                                    directions, hint)
+        rgb = out.get("rgb")
+        ctx.save_for_backward(out["cell"], directions, rgb)
+        ctx.pipeline, ctx.num_points = pipeline, points.shape[0]
+        ctx.mark_non_differentiable(out["cell"])
+        return out["density"], rgb, out["cell"]
+
+    @staticmethod
+    def backward(ctx, grad_density, grad_rgb, _grad_cell):
+        cell, directions, rgb = ctx.saved_tensors
+        attr_grad = None
+        if ctx.needs_input_grad[2]:
+            attr_grad = ctx.pipeline.sample_field_backward(ctx.num_points, cell, directions, rgb,
+                                                           None if rgb is None else grad_rgb, grad_density)
+        ctx.pipeline = None
+        return None, None, attr_grad, None, None, None, None, None
+
+
 class TraceRaysParams(torch.autograd.Function):
     """The render op taken one step further out: ``RadFoamScene.forward`` = ``get_trace_data`` (a ``cat`` and a
     softplus, scene.py:202-217) followed by ``TraceRays`` (scene.py:236-261).  Here the model's PARAMETERS go in --
