@@ -756,8 +756,10 @@ __global__ void __launch_bounds__(kBlock) backward_kernel(const BackwardParams p
 // sliver cell the other misses and they drift out of lock-step), so instead of 13 x 128-bit
 // reductions per lane per step the warp keeps a small direct-mapped cache of gradient rows in
 // shared memory:
-//   * every lane with a row this step writes it (SH products + density grad) to its own
-//     staging row in shared memory;
+//   * a composited step's row is held in registers until the lane's next composited step, which
+//     finishes that cell's position gradient (BackwardRay::cell flushes it one cell late); then
+//     the lane writes the row (SH products, density grad, position grad) to its own staging row
+//     in shared memory, so the position gradient needs no reduction of its own;
 //   * lanes are grouped by cell (MATCH.ANY); a lane in a group of fewer than MIN_GROUP lanes
 //     sends its staged row to HBM as one bulk reduction (cp.reduce.async.bulk: the TMA unit reads
 //     the row, so the LSU issues no request per 16 bytes), and waits for that read to finish only
@@ -767,7 +769,6 @@ __global__ void __launch_bounds__(kBlock) backward_kernel(const BackwardParams p
 //     and has no bank conflicts, and adds the sum to the cell's cache row;
 //   * a cache row is written to HBM (13 lanes x one RED.128) only when its slot is claimed by
 //     another cell, or when the warp's rays are finished.
-// Position gradients (3 floats to the previous composited cell) stay direct reductions.
 // MIN_GROUP: smallest same-cell lane group routed through the cache (smaller groups send one
 // bulk reduction per lane, which costs fewer issue slots than one serial cache round per group,
 // at the price of more L2 atomic traffic).
@@ -864,11 +865,19 @@ __global__ void __launch_bounds__(kBlock, MIN_BLOCKS * 128 / kBlock)
             G[k] = 0.0f;
     }
 
+    // the row of this lane's last composited cell, held until the lane's next composited step has finished that
+    // cell's position gradient (BackwardRay::cell flushes it one cell late), so that the row and its position
+    // gradient leave together; a ray's last row leaves with zero position slots once the ray is done
+    uint32_t p_cell = kNone;
+    float p_ds = 0.0f;
+    float p_drgb[3] = {0.0f, 0.0f, 0.0f};
+
     for (uint32_t k = 0;; ++k) {
-        bool c_valid = false; // this lane has a (SH, density) row for cell c_cell this iteration
+        bool c_valid = false; // this lane has a row for cell c_cell this iteration
         uint32_t c_cell = kNone;
         float dL_ds = 0.0f;
         float dL_drgb[3] = {0.0f, 0.0f, 0.0f};
+        float fx = 0.0f, fy = 0.0f, fz = 0.0f; // c_cell's position gradient
 
         // one step of the ray: (cur, t1, nxt) from the tape, or from scanning the cell's faces
         bool step = false;
@@ -911,19 +920,27 @@ __global__ void __launch_bounds__(kBlock, MIN_BLOCKS * 128 / kBlock)
                 float rgb[3] = {0.0f, 0.0f, 0.0f};
                 if (pc.w > 1e-6f)
                     sh_to_rgb<DEG>(p.sh_rows + (uint64_t)cur * SR, sh, rgb[0], rgb[1], rgb[2]);
-                float w, fx, fy, fz;
+                float w, n_ds, n_drgb[3];
                 bool flush;
                 uint32_t flush_idx;
-                bool go = st.template cell<RAY>(cur, pc, pn, t0, t1, rgb, ray, p.weight_threshold, dL_drgb,
-                                                dL_ds, w, flush, flush_idx, fx, fy, fz, ra);
+                bool go = st.template cell<RAY>(cur, pc, pn, t0, t1, rgb, ray, p.weight_threshold, n_drgb, n_ds,
+                                                w, flush, flush_idx, fx, fy, fz, ra);
                 if (RAY)
-                    sh_grad_contract<DEG>(p.sh_rows + (uint64_t)cur * SR, dL_drgb, G);
+                    sh_grad_contract<DEG>(p.sh_rows + (uint64_t)cur * SR, n_drgb, G);
                 if (p.point_error)
                     add_point_error(p, cur, __fmul_rn(w, st.err));
-                if (flush)
-                    red_add_v4(p.acc + (uint64_t)flush_idx * GR + SR, 0.0f, fx, fy, fz);
-                c_valid = true;
-                c_cell = cur;
+                // every composited step sets st.prev, so flush == (p_cell != kNone) and flush_idx == p_cell:
+                // the held row leaves now, carrying its finished position gradient
+                c_valid = flush;
+                c_cell = p_cell;
+                dL_ds = p_ds;
+#pragma unroll
+                for (int c = 0; c < 3; ++c) {
+                    dL_drgb[c] = p_drgb[c];
+                    p_drgb[c] = n_drgb[c];
+                }
+                p_cell = cur;
+                p_ds = n_ds;
                 done = !go;
             }
             t0 = fmaxf(t0, t1);
@@ -931,6 +948,18 @@ __global__ void __launch_bounds__(kBlock, MIN_BLOCKS * 128 / kBlock)
             pc = pn;
             if (replay && k + 1 >= nrec)
                 done = true;
+        }
+        if (!c_valid && done && p_cell != kNone) {
+            // the ray is done: its last composited cell's row leaves with zero position slots (that cell's
+            // position gradient is never finished: quirk A.5.1)
+            c_valid = true;
+            c_cell = p_cell;
+            dL_ds = p_ds;
+#pragma unroll
+            for (int c = 0; c < 3; ++c)
+                dL_drgb[c] = p_drgb[c];
+            fx = fy = fz = 0.0f;
+            p_cell = kNone;
         }
 
         // ---- warp-collective phase: route this iteration's rows
@@ -948,7 +977,7 @@ __global__ void __launch_bounds__(kBlock, MIN_BLOCKS * 128 / kBlock)
                     v[k] = (i + k < 3 * sh_dim(DEG)) ? __fmul_rn(sh[(i + k) / 3], dL_drgb[(i + k) % 3]) : 0.0f;
                 srow[i / 4] = make_float4(v[0], v[1], v[2], v[3]);
             }
-            srow[SR / 4] = make_float4(dL_ds, 0.0f, 0.0f, 0.0f);
+            srow[SR / 4] = make_float4(dL_ds, fx, fy, fz);
         }
         if (single) {
             // the whole row as one bulk reduction; a row whose three channel gradients are all zero sends
@@ -1013,7 +1042,7 @@ __global__ void __launch_bounds__(kBlock, MIN_BLOCKS * 128 / kBlock)
                 __syncwarp();
             }
         }
-        if (!__any_sync(FULL, !done))
+        if (!__any_sync(FULL, !done || p_cell != kNone))
             break;
     }
 

@@ -526,11 +526,14 @@ int launch_backward_cached_cfg(const BackwardParams &bp, const Faces &fa, const 
 // (<= 102 registers; the H100's 64 K registers per SM hold 5 CTAs of 128 threads at 96).  Fewer slots keep the
 // per-warp staging small; 6 CTAs/SM would spill.  With 4 slots a CTA needs under 32 KB of shared memory, so 5 CTAs
 // take about 150 KB of the H100's 228 KB per SM and the rest stays L1.
+// Degree 3 gets 4 CTAs/SM (<= 128 registers): the row each lane holds until its next composited step (five values
+// live across the step) made the 96-register build spill 108 bytes, and at 4 CTAs/SM the replay backward is 5 %
+// faster on the bench frame (profiles/h100_backward_position_fold.json).
 // With ray gradients (RAY) each thread also keeps its ray's sums (the G_k alone are (deg+1)^2 registers): those
 // instantiations get fewer CTAs/SM, so that they do not spill -- 4 (<= 128 registers) for degrees 0-2 and 3
 // (<= 168) for degree 3, which spills at 128.
 template <int DEG, bool RAY>
-constexpr int backward_min_blocks() { return !RAY ? 5 : DEG == 3 ? 3 : 4; }
+constexpr int backward_min_blocks() { return !RAY ? (DEG == 3 ? 4 : 5) : DEG == 3 ? 3 : 4; }
 template <typename Faces>
 int launch_backward_cached(int deg, const BackwardParams &bp, const Faces &fa, const Tape &tape,
                            const RayGradOut &rg, uint32_t blocks, cudaStream_t stream) {
