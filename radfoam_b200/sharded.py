@@ -57,10 +57,13 @@ def unshard_image(parts: list[torch.Tensor], height: int, band: int = 8) -> torc
     world = len(parts)
     if world == 1:
         return parts[0]
+    dtype = parts[0].dtype
+    if dtype == torch.uint32:  # index_copy_ has no uint32 kernel: move the same bits as int32
+        parts = [p.view(torch.int32) for p in parts]
     out = torch.empty((height,) + tuple(parts[0].shape[1:]), dtype=parts[0].dtype, device=parts[0].device)
     for r, p in enumerate(parts):
         out.index_copy_(0, band_rows(height, r, world, band).to(p.device), p)
-    return out
+    return out.view(dtype)
 
 
 class ShardedTracer:

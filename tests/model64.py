@@ -724,14 +724,15 @@ def rows_reachable(m: dict, offsets, adjacency, points, attributes, rays, start,
 
 def check_implementation(impl, points, attributes, adjacency, offsets, rays, start, quantiles, grad_rgba,
                          grad_depth, ray_error=None, weight_threshold=0.001, max_intersections=1024,
-                         contribution=True, half_atomics=False) -> dict:
+                         contribution=True, half_atomics=False, return_model=False):
     """Trace a case with an implementation and hold every output to the model.
 
     ``impl(rays, start, quantiles, grad_rgba, grad_depth, ray_error, backward)`` returns numpy outputs of
     the forward (with contribution) and, with ``backward``, of the backward on its own saved rgba and depth
     indices.  Ambiguous rays get zero upstream gradients and ray error in both the model and the
     implementation, so the image and its layout stay as given; where any exist, ``contribution`` (a
-    forward output) is compared on a flat batch of the unambiguous rays instead."""
+    forward output) is compared on a flat batch of the unambiguous rays instead.  Returns the tightness
+    report, or ``(report, model)`` with ``return_model`` (to hold further outputs to the same model)."""
     settings = (weight_threshold, max_intersections)
     scene = (points, attributes, adjacency, offsets)
     m0 = trace(*scene, rays, start, quantiles, *settings, backward=False)
@@ -755,7 +756,7 @@ def check_implementation(impl, points, attributes, adjacency, offsets, rays, sta
         flat = impl(r, s, q, None, None, None, False)
         mf = trace(*scene, r, s, q, *settings, backward=False)
         report["contribution"] = compare({"contribution": flat["contribution"]}, mf, per_ray=False)["contribution"]
-    return report
+    return (report, m) if return_model else report
 
 
 def format_report(name: str, report: dict) -> str:
