@@ -24,6 +24,7 @@ import test_gpu_fullsize as fullsize  # noqa: E402
 import test_gpu_fuzz as fuzz  # noqa: E402
 import test_gpu_parity as parity  # noqa: E402
 import test_gpu_reference_op as reference_op  # noqa: E402
+import test_gpu_stale_model64 as stale  # noqa: E402
 from oracle import ref_gpu  # noqa: E402
 
 
@@ -99,6 +100,20 @@ def make_fullsize():
     return {"config2": fullsize.reference_record(world)}
 
 
+def make_stale():
+    """Stale scenes (moved points, the adjacency kept): integers whole, floats and gradients on sampled rows, and the
+    reference's run-to-run gradient noise."""
+    recs = {}
+    for name, make in stale.REF_CASES.items():
+        case = make()
+        ref = parity.run_ref_gpu(torch, case)
+        recs[name] = refgold.record(ref, exact=parity.REF_EXACT, sampled=[k for k in parity.REF_SAMPLED if k in ref])
+        ref2 = parity.run_ref_gpu(torch, case)
+        recs[name]["grad_noise"] = np.float64(max(common.grad_error(ref2[k], ref[k])
+                                                  for k in ("points_grad", "attr_grad")))
+        print(name, "reference noise", float(recs[name]["grad_noise"]), flush=True)
+    return recs
+
 
 def main(outdir):
     import pathlib
@@ -107,7 +122,7 @@ def main(outdir):
     assert ref_gpu.available(), "oracle/_ref is not built"
     os.makedirs(outdir, exist_ok=True)
     groups = {"parity": lambda: make_parity(pathlib.Path(tempfile.mkdtemp())), "fuzz": make_fuzz, "farthest": make_farthest,
-              "reference_op": make_reference_op, "fullsize": make_fullsize, "configs": make_configs}
+              "reference_op": make_reference_op, "fullsize": make_fullsize, "configs": make_configs, "stale": make_stale}
     only = sys.argv[2:] or list(groups)
     for name in only:
         recs = groups[name]()

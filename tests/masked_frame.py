@@ -107,7 +107,7 @@ class MaskedFrame:
 
 
 def check_paths(scene, frame: MaskedFrame, grad_rgba, grad_depth, ray_error, runs: dict, weight_threshold=0.001,
-                max_intersections=1024, half_atomics=False) -> dict:
+                max_intersections=1024, half_atomics=False, model=None) -> dict:
     """Hold every full-frame run in ``runs`` to one model result for S.
 
     ``scene`` = (points, attributes, adjacency, offsets); ``grad_rgba``, ``grad_depth``, ``ray_error`` are S's
@@ -117,7 +117,8 @@ def check_paths(scene, frame: MaskedFrame, grad_rgba, grad_depth, ray_error, run
 
     As in ``model64.check_implementation``, S's ambiguous rays get zero upstream.  The model (with ray gradients)
     runs once, on the first run's rgba and depth indices; every later run's forward outputs on S must be
-    bit-identical to the first's.  Returns {name: model64 report}."""
+    bit-identical to the first's.  Returns {name: model64 report}; ``model`` (a dict), if given, receives the model
+    result for S."""
     rays, start, dq = frame.batch(frame.rays), frame.batch(frame.start), frame.batch(frame.quantiles)
     settings = (weight_threshold, max_intersections)
     amb = MR.trace(*scene, rays, start, dq, *settings, backward=False)["ambiguous"]
@@ -133,6 +134,8 @@ def check_paths(scene, frame: MaskedFrame, grad_rgba, grad_depth, ray_error, run
             m = MR.trace(*scene, rays, start, dq, *settings, rgba=got["rgba"], grad_rgba=g, grad_depth=gd,
                          depth_indices=got.get("depth_indices"), ray_error=err, ray_grad=True)
             assert np.array_equal(m["ambiguous"], amb)
+            if model is not None:
+                model.update(m)
         else:
             for k in FORWARD:
                 if k in first:

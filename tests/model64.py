@@ -256,7 +256,10 @@ def trace(points, attributes, adjacency, offsets, rays, start, quantiles=None, w
     The backward is defined on the forward's saved ``rgba`` -- pass the output of the implementation
     under test; ``None`` uses the model's own (what a finite-difference check needs).  ``depth_indices``
     likewise (``None``: the model's).  Returns a dict: per-ray outputs ``rgba``, ``depth`` (each with an
-    ``*_err`` bound), ``depth_indices``, ``num_intersections``, ``ambiguous``; ``Scatter`` objects
+    ``*_err`` bound), ``depth_indices``, ``num_intersections``, ``ambiguous``; per-ray walk statistics
+    ``skipped`` (a cell was skipped with t1 <= t0), ``composited`` (cells composited), ``reentered`` (composited
+    cells not entered through the previous composited cell's exit plane, i.e. after skipped cells) and
+    ``stuck_cell`` (the cell where the walk found no face with dp > 0, -1 if it ended otherwise); ``Scatter`` objects
     ``contribution``, ``points_grad``, ``attr_grad`` and (with ``ray_error``) ``point_error``."""
     if backward and (rgba is None or depth_indices is None):
         fwd = trace(points, attributes, adjacency, offsets, rays, start, quantiles, weight_threshold,
@@ -284,7 +287,8 @@ def trace(points, attributes, adjacency, offsets, rays, start, quantiles=None, w
     out = dict(rgba=np.zeros((r_all, 4)), rgba_err=np.zeros((r_all, 4)),
                num_intersections=np.zeros(r_all, dtype=np.uint32), ambiguous=np.zeros(r_all, dtype=bool),
                first_cell=np.full(r_all, -1), last_cell=np.full(r_all, -1), last_next=np.full(r_all, -1),
-               skipped=np.zeros(r_all, dtype=bool))
+               skipped=np.zeros(r_all, dtype=bool), composited=np.zeros(r_all, dtype=np.int64),
+               reentered=np.zeros(r_all, dtype=np.int64), stuck_cell=np.full(r_all, -1))
     if q_n:
         out.update(depth=np.full((r_all, q_n), -1.0), depth_err=np.zeros((r_all, q_n)),
                    depth_indices=np.full((r_all, q_n), NONE, dtype=np.uint32))
@@ -318,6 +322,8 @@ def trace(points, attributes, adjacency, offsets, rays, start, quantiles=None, w
         amb = np.zeros(rc, dtype=bool)
         first_cell, last_cell, last_next = np.full(rc, -1), np.full(rc, -1), np.full(rc, -1)
         skipped = np.zeros(rc, dtype=bool)
+        composited, reentered = np.zeros(rc, dtype=np.int64), np.zeros(rc, dtype=np.int64)
+        stuck_cell = np.full(rc, -1)
         active = np.ones(rc, dtype=bool)
         depth = np.full((rc, q_n), -1.0)
         depth_e = np.zeros((rc, q_n))
@@ -358,6 +364,7 @@ def trace(points, attributes, adjacency, offsets, rays, start, quantiles=None, w
             nf = off[c_cur + 1] - b
             F = int(nf.max())
             if F == 0:
+                stuck_cell[a] = cur[a]
                 active[a] = False
                 break
             cols = b[:, None] + np.arange(F)
@@ -392,6 +399,7 @@ def trace(points, attributes, adjacency, offsets, rays, start, quantiles=None, w
                 rival = cand & notwin & ~(t > t1v[:, None] + 2 * (e_t + t1e[:, None]))
             amb_step = np.where(found, rival.any(1) | unsure_dp[ri, win], cand.any(1))
             amb[a] |= amb_step
+            stuck_cell[a[~found]] = cur[a[~found]]
             active[a[~found]] = False
             a, win, t1v, t1e = a[found], win[found], t1v[found], t1e[found]
             if a.size == 0:
@@ -405,6 +413,8 @@ def trace(points, attributes, adjacency, offsets, rays, start, quantiles=None, w
             skipped[a[~comp]] = True
             if cidx.size:
                 first_cell[cidx] = np.where(first_cell[cidx] < 0, cur[cidx], first_cell[cidx])
+                reentered[cidx] += (last_next[cidx] >= 0) & (last_next[cidx] != cur[cidx])
+                composited[cidx] += 1
                 last_cell[cidx], last_next[cidx] = cur[cidx], nxt[comp]
                 cont = _cell(locals())
                 active[cidx[~cont]] = False
@@ -425,6 +435,7 @@ def trace(points, attributes, adjacency, offsets, rays, start, quantiles=None, w
         out["ambiguous"][sel] = amb
         out["first_cell"][sel], out["last_cell"][sel], out["last_next"][sel] = first_cell, last_cell, last_next
         out["skipped"][sel] = skipped
+        out["composited"][sel], out["reentered"][sel], out["stuck_cell"][sel] = composited, reentered, stuck_cell
         if q_n:
             out["depth"][sel] = depth
             out["depth_err"][sel] = depth_e
@@ -438,7 +449,8 @@ def trace(points, attributes, adjacency, offsets, rays, start, quantiles=None, w
 
     res = {k: v.reshape(batch + v.shape[1:]) for k, v in out.items()}
     res["num_intersections"] = res["num_intersections"].reshape(batch + (1,))
-    for k in ("ambiguous", "first_cell", "last_cell", "last_next", "skipped"):
+    for k in ("ambiguous", "first_cell", "last_cell", "last_next", "skipped", "composited", "reentered",
+              "stuck_cell"):
         res[k] = out[k].reshape(batch)
     res["contribution"] = contribution
     if backward:

@@ -111,7 +111,8 @@ def trace(points, attributes, adjacency, offsets, rays, start, quantiles=None, w
     out = dict(rgba=np.zeros((r_all, 4)), rgba_err=np.zeros((r_all, 4)),
                num_intersections=np.zeros(r_all, dtype=np.uint32), ambiguous=np.zeros(r_all, dtype=bool),
                first_cell=np.full(r_all, -1), last_cell=np.full(r_all, -1), last_next=np.full(r_all, -1),
-               skipped=np.zeros(r_all, dtype=bool))
+               skipped=np.zeros(r_all, dtype=bool), composited=np.zeros(r_all, dtype=np.int64),
+               reentered=np.zeros(r_all, dtype=np.int64), stuck_cell=np.full(r_all, -1))
     if q_n:
         out.update(depth=np.full((r_all, q_n), -1.0), depth_err=np.zeros((r_all, q_n)),
                    depth_indices=np.full((r_all, q_n), NONE, dtype=np.uint32))
@@ -147,6 +148,8 @@ def trace(points, attributes, adjacency, offsets, rays, start, quantiles=None, w
         amb = np.zeros(rc, dtype=bool)
         first_cell, last_cell, last_next = np.full(rc, -1), np.full(rc, -1), np.full(rc, -1)
         skipped = np.zeros(rc, dtype=bool)
+        composited, reentered = np.zeros(rc, dtype=np.int64), np.zeros(rc, dtype=np.int64)
+        stuck_cell = np.full(rc, -1)
         active = np.ones(rc, dtype=bool)
         depth = np.full((rc, q_n), -1.0)
         depth_e = np.zeros((rc, q_n))
@@ -192,6 +195,7 @@ def trace(points, attributes, adjacency, offsets, rays, start, quantiles=None, w
             nf = off[c_cur + 1] - b
             F = int(nf.max())
             if F == 0:
+                stuck_cell[a] = cur[a]
                 active[a] = False
                 break
             cols = b[:, None] + np.arange(F)
@@ -226,6 +230,7 @@ def trace(points, attributes, adjacency, offsets, rays, start, quantiles=None, w
                 rival = cand & notwin & ~(t > t1v[:, None] + 2 * (e_t + t1e[:, None]))
             amb_step = np.where(found, rival.any(1) | unsure_dp[ri, win], cand.any(1))
             amb[a] |= amb_step
+            stuck_cell[a[~found]] = cur[a[~found]]
             active[a[~found]] = False
             a, win, t1v, t1e = a[found], win[found], t1v[found], t1e[found]
             if a.size == 0:
@@ -239,6 +244,8 @@ def trace(points, attributes, adjacency, offsets, rays, start, quantiles=None, w
             skipped[a[~comp]] = True
             if cidx.size:
                 first_cell[cidx] = np.where(first_cell[cidx] < 0, cur[cidx], first_cell[cidx])
+                reentered[cidx] += (last_next[cidx] >= 0) & (last_next[cidx] != cur[cidx])
+                composited[cidx] += 1
                 last_cell[cidx], last_next[cidx] = cur[cidx], nxt[comp]
                 cont = _cell(locals())
                 active[cidx[~cont]] = False
@@ -259,6 +266,7 @@ def trace(points, attributes, adjacency, offsets, rays, start, quantiles=None, w
         out["ambiguous"][sel] = amb
         out["first_cell"][sel], out["last_cell"][sel], out["last_next"][sel] = first_cell, last_cell, last_next
         out["skipped"][sel] = skipped
+        out["composited"][sel], out["reentered"][sel], out["stuck_cell"][sel] = composited, reentered, stuck_cell
         if q_n:
             out["depth"][sel] = depth
             out["depth_err"][sel] = depth_e
@@ -274,7 +282,8 @@ def trace(points, attributes, adjacency, offsets, rays, start, quantiles=None, w
 
     res = {k: v.reshape(batch + v.shape[1:]) for k, v in out.items()}
     res["num_intersections"] = res["num_intersections"].reshape(batch + (1,))
-    for k in ("ambiguous", "first_cell", "last_cell", "last_next", "skipped"):
+    for k in ("ambiguous", "first_cell", "last_cell", "last_next", "skipped", "composited", "reentered",
+              "stuck_cell"):
         res[k] = out[k].reshape(batch)
     res["contribution"] = contribution
     if backward:

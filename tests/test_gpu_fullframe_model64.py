@@ -43,13 +43,17 @@ def _quiet():
 class Frame:
     """A foam on the device and one camera's full frame, with a seeded upstream of the common.Case kind."""
 
-    def __init__(self, torch, num_points, width, height, attr_dtype=np.float32, **settings):
+    def __init__(self, torch, num_points, width, height, attr_dtype=np.float32, points=None, **settings):
+        """``points``: trace the foam with these points instead of its own (a stale foam: moved points, the same
+        adjacency); the camera's start cell is their nearest point."""
         import bench
         import radfoam_b200
         from radfoam_b200 import foam
 
         self.torch, self.settings, self.attr_dtype = torch, settings, attr_dtype
         f = self.foam = bench.load_or_build_foam(num_points, lambda m: None)
+        if points is not None:
+            f = self.foam = foam.Foam(points, f.attributes, f.adjacency, f.offsets, f.sh_degree)
         self.scene = (f.points, f.attributes.astype(attr_dtype), f.adjacency, f.offsets)
         rays = foam.pinhole_rays(width, height, CAMERA, fov=0.9)
         start = np.full((height, width), foam.nearest_point(f.points, CAMERA), dtype=np.uint32)
@@ -103,12 +107,12 @@ class Frame:
             return out
         return run
 
-    def check(self, name, sel, runs):
+    def check(self, name, sel, runs, model=None):
         frame = MF.MaskedFrame(self.case.rays, self.case.start, self.case.quantiles, sel)
         t = time.perf_counter()
         reports = MF.check_paths(self.scene, frame, frame.batch(self.case.grad_rgba.astype(self.attr_dtype)),
                                  frame.batch(self.case.grad_depth), frame.batch(self.ray_error), runs,
-                                 **self.settings)
+                                 model=model, **self.settings)
         dt = time.perf_counter() - t
         for path, report in reports.items():
             print("\n" + M.format_report(f"{name} {path}", report))

@@ -406,12 +406,10 @@ def test_nearest_point_and_starting_points(torch_cuda):
     rng = np.random.default_rng(2)
     queries = np.concatenate([rng.normal(0, 2.0, size=(257, 3)), f.points[:5].astype(np.float64)]).astype(np.float32)
     got = radfoam_b200.nearest_point(to_dev(torch, f.points), to_dev(torch, queries)).cpu().numpy()
-    d2 = ((f.points[None, :, :].astype(np.float64) - queries[:, None, :].astype(np.float64)) ** 2).sum(-1)
-    want = d2.argmin(axis=1)
-    # exact up to fp32-vs-fp64 near-ties: the chosen point must be (numerically) as close as the best
-    chosen = d2[np.arange(len(queries)), got.astype(np.int64)]
-    assert (chosen <= d2.min(axis=1) * (1 + 1e-5) + 1e-12).all()
-    assert (got.astype(np.int64) == want).mean() > 0.99
+    # the contract exactly (smallest fp32 distance, ties to the lowest index), and cKDTree away from fp32 near-ties
+    from test_gpu_entry_cells import check_nearest
+
+    check_nearest(torch, f.points, queries, got)
     assert np.array_equal(got[-5:], np.arange(5))        # a point is its own nearest point
     # per-ray start cells: one frame (single origin) and a multi-camera batch
     case = common.scene_case(num_points=60000, width=320, height=200)

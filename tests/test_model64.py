@@ -270,6 +270,52 @@ def test_emulated_kernels_small_scene_within_model_bounds(tape, monkeypatch):
     print("\n" + M.format_report(f"emu scene1500 tape={tape}", report))
 
 
+def test_walk_statistics():
+    """The per-ray walk statistics stale scenes are judged by: one composited cell per contribution term; a cell can
+    only be re-entered (not through the previous composited cell's exit plane) after a skipped cell, and not the
+    first; ``stuck_cell`` is set exactly on the rays that neither ran out of steps nor fell to the weight threshold,
+    and no face of it lies in front of the ray.  On a fresh triangulation nothing is re-entered and walks only stop
+    without an exit face on the hull; on the same foam with moved points both happen."""
+    from scipy.spatial import ConvexHull
+
+    import stale_cases as S
+
+    fresh = common.config1(3, 2)
+    for case in (fresh, S.stale_case(fresh, 0.5, "noise", seed=1)):
+        f = case.foam
+        faces = M.face_offsets(f.points, f.adjacency, f.offsets)
+        off = f.offsets.astype(np.int64)
+        d = case.rays.reshape(-1, 6)[:, 3:].astype(np.float64)
+        d /= np.linalg.norm(d, axis=1, keepdims=True)
+        for budget in (1024, 6):
+            m = M.trace(f.points, f.attributes, f.adjacency, f.offsets, case.rays, case.start, case.quantiles,
+                        max_intersections=budget, backward=False)
+            assert m["composited"].sum() == m["contribution"].count.sum() > 0
+            assert (m["reentered"] <= np.maximum(m["composited"] - 1, 0)).all()
+            assert not m["reentered"][~m["skipped"]].any()
+            stuck = m["stuck_cell"].reshape(-1)
+            out_of_steps = m["num_intersections"].reshape(-1) == budget + 1
+            transmittance = 1.0 - m["rgba"].reshape(-1, 4)[:, 3]
+            thr = float(np.float32(0.001))
+            faded = transmittance <= thr * (1 + 1e-9)
+            assert np.array_equal(stuck >= 0, ~out_of_steps & ~faded)
+            assert (transmittance[stuck >= 0] > thr).all()
+            for r in np.flatnonzero(stuck >= 0):
+                assert (faces[off[stuck[r]]:off[stuck[r] + 1]] @ d[r] <= 0).all(), r
+            if budget < 1024:
+                assert out_of_steps.any()
+                continue
+            assert (stuck >= 0).any() and faded.any()
+            hull = np.zeros(f.num_points, dtype=bool)
+            hull[ConvexHull(f.points.astype(np.float64)).vertices] = True
+            inside = (stuck >= 0) & ~hull[np.maximum(stuck, 0)]
+            if case is fresh:
+                assert not m["skipped"].any() and not m["reentered"].any() and not inside.any()
+            else:
+                assert m["reentered"].sum() > 0 and inside.sum() > 0
+                assert S.stats(m, f.points).stranded == int(inside.sum())
+
+
 def test_compare_fp16_overflow_to_inf():
     """An fp16 scatter entry whose sum reaches 65520 rounds to inf of its sign; a wrong sign, or inf where the bound
     stays below the overflow, is still a mismatch."""
