@@ -14,6 +14,7 @@
  *   rfb_trace_visualization <- Pipeline::trace_visualization src/tracing/pipeline.h:102-115
  *   rfb_locate_points        <- radfoam::nn over the AABB tree  src/aabb_tree/aabb_tree.cu:343-415 (any number of queries)
  *   rfb_sample_field(_backward)  (new) the field at arbitrary points and its attribute gradient
+ *   rfb_surface_count/_write     (new) the Voronoi faces between occupied and empty cells, as polygons
  *
  * The reference interface is a C++ vtable taking raw device pointers (Eigen
  * types appear only as reinterpret_casts of packed floats); this header
@@ -220,6 +221,45 @@ int rfb_sample_field_backward(rfb_pipeline *pipeline, uint32_t num_points, uint3
                               const uint32_t *cells, const float *directions, const void *rgb,
                               const void *rgb_grad, const void *density_grad, void *attribute_grad,
                               void *stream);
+
+/* ---- surface extraction: the Voronoi faces between occupied and empty cells ----
+ * Definition.  For row i of the CSR and every listed neighbour k with p_k != p_i let
+ *   H_k = { x : (p_k - p_i).x <= (p_k - p_i).(p_i + p_k)/2 },   C_i = the intersection of the box and every H_k,
+ * the region the walk treats as cell i (it leaves i through the nearest of these planes): on a Delaunay adjacency
+ * the box-clipped Voronoi cell, on a stale one the tracer's restricted cell.  Each CSR entry e = (i, j) yields the
+ * polygon F_e = C_i intersected with plane_e (the boundary of H_j), emitted iff inside[i] && !inside[j], p_j != p_i and F_e has at least 3 vertices.
+ * Output order is CSR order and repeated calls give identical bytes; a repeated CSR entry yields a repeated
+ * polygon, and nothing is welded or deduplicated across polygons.  Vertices are counter-clockwise seen from the j
+ * side (the right-hand normal points out of the occupied cell), computed in float64 and rounded once to float32.
+ * rgb of a polygon = the colour of cell i along normalize(p_i - p_j) -- what a ray entering i through the face
+ * sees --, bit-identical to rfb_sample_field with that direction for a query located in i.
+ * Limits: the surface is open where occupied cells reach the box (no caps are emitted); on a stale adjacency the
+ * polygons follow the definition but need not close.  A polygon needing more than 32 vertices is not emitted and
+ * counted in totals[2]: a caller must treat that as an error, never as a short surface.
+ * Preconditions: a valid CSR (offsets[0] = 0, non-decreasing, offsets[N] = E) and a finite box with lo <= hi.
+ *
+ * Two passes, both allocation-free, neither touching a pipeline's scene mirrors, walk tape or accumulator:
+ *   rfb_surface_count  fills `scratch` (rfb_surface_scratch_bytes(E) bytes of device memory, any contents): it
+ *     starts with uint64 totals[4] = {vertices V, polygons P, polygons over the vertex capacity, 0}, followed by the
+ *     per-entry exclusive offsets;
+ *   rfb_surface_write  (same geometry arguments, the scratch of that count) writes vertices[V][3] f32,
+ *     offsets[P+1] int64 (polygon k = vertices [offsets[k], offsets[k+1])), cells[P][2] u32 = (i, j) and rgb[P][3]
+ *     in the pipeline's attribute dtype (its SH degree).  It writes only the vertex runs and slots the count
+ *     assigned (vertices, cells and rgb may be NULL when P = 0).  Sizing the outputs needs the totals on the host:
+ *     a caller synchronises between the two. */
+typedef struct rfb_box {
+    float lo[3];
+    float hi[3];
+} rfb_box;
+uint64_t rfb_surface_scratch_bytes(uint32_t point_adjacency_size);
+int rfb_surface_count(const float *points, uint32_t num_points, uint32_t point_adjacency_size,
+                      const uint32_t *point_adjacency, const uint32_t *point_adjacency_offsets,
+                      const uint8_t *inside, const rfb_box *bounds, void *scratch, void *stream);
+int rfb_surface_write(rfb_pipeline *pipeline, const float *points, uint32_t num_points, const void *attributes,
+                      uint32_t point_adjacency_size, const uint32_t *point_adjacency,
+                      const uint32_t *point_adjacency_offsets, const uint8_t *inside, const rfb_box *bounds,
+                      const void *scratch, float *vertices, int64_t *offsets, uint32_t *cells, void *rgb,
+                      void *stream);
 
 int rfb_trace_forward(rfb_pipeline *pipeline, const rfb_trace_settings *settings,
                       uint32_t num_points, const float *points,

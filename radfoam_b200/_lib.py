@@ -36,6 +36,10 @@ class Multicast(ctypes.Structure):  # rfb_multicast
     _fields_ = [("acc", c_void_p), ("attribute_grad", c_void_p), ("points_grad", c_void_p)]
 
 
+class Box(ctypes.Structure):  # rfb_box
+    _fields_ = [("lo", c_float * 3), ("hi", c_float * 3)]
+
+
 class LaunchOpts(ctypes.Structure):  # rfb_launch_opts
     _fields_ = [("scene_version", c_uint64), ("image_width", c_uint32), ("flags", c_uint32)]
 
@@ -73,6 +77,10 @@ SIGNATURES = {
     "rfb_locate_points": (c_int, [_P, c_uint32, _P, _P, _P, c_uint32, _P, _P, _P]),
     "rfb_sample_field": (c_int, [_P, _P, c_uint32, _P, _P, _P, _P, c_uint32, _P, _P, _P, _P, _P, _P]),
     "rfb_sample_field_backward": (c_int, [_P, c_uint32, c_uint32, _P, _P, _P, _P, _P, _P, _P]),
+    "rfb_surface_scratch_bytes": (c_uint64, [c_uint32]),
+    "rfb_surface_count": (c_int, [_P, c_uint32, c_uint32, _P, _P, _P, POINTER(Box), _P, _P]),
+    "rfb_surface_write": (c_int, [_P, _P, c_uint32, _P, c_uint32, _P, _P, _P, POINTER(Box), _P, _P, _P, _P, _P,
+                                  _P]),
     "rfb_trace_forward": (c_int, [_P, POINTER(TraceSettings), c_uint32, _P, _P, c_uint32, _P, _P,
                                   c_uint32, _P, _P, c_uint32, _P, _P, _P, _P, _P, _P,
                                   POINTER(LaunchOpts), _P]),

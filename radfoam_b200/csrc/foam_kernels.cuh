@@ -1934,4 +1934,370 @@ __global__ void __launch_bounds__(kBlock) visualization_kernel(const Visualizati
     out.store(pi, row, v);
 }
 
+// ------------------------------------------------------------------ surface extraction (rfb_surface_count / _write)
+// Cell C_i = box ∩ { x : (p_k - p_i).x <= (p_k - p_i).(p_i + p_k)/2 } over the neighbours k of row i with p_k != p_i:
+// the region the walk treats as cell i.  For CSR entry e = (i, j) with inside[i], !inside[j] and p_j != p_i the
+// polygon F_e = C_i ∩ plane_e, vertices counter-clockwise seen from j.  Geometry in fp64, rounded once to fp32.
+// Both passes run a warp per row (the row's entries on its lanes; rows that are not inside leave at once) and get
+// every polygon from surface_polygon, so the write pass reproduces the count pass's vertex counts exactly.
+constexpr int kSurfaceMaxVerts = 32; // a polygon that needs more fails the call (kernel-local ping-pong buffers)
+constexpr int kSurfaceBlock = 256;   // 8 rows per CTA
+constexpr int kScanBlock = 256, kScanItems = 4, kScanTile = kScanBlock * kScanItems;
+
+struct SurfaceParams {
+    const float *points;
+    const uint32_t *adj;
+    const uint32_t *off;
+    const uint8_t *inside;
+    uint32_t num_points, num_entries;
+    float lo[3], hi[3];
+};
+
+// Keeps the part of `in` (n vertices) where (x - m).nrm <= 0, vertex order preserved (Sutherland-Hodgman).  A new
+// vertex is made only where an edge crosses the plane strictly, so a vertex on the plane is never doubled.  Returns
+// the vertex count, or -1 when it would exceed kSurfaceMaxVerts.  NaN distances drop their vertices.
+__device__ __forceinline__ int clip_polygon(const double (*in)[3], int n, double (*out)[3], const double *nrm,
+                                            const double *m) {
+    if (n == 0)
+        return 0;
+    auto dist = [&](const double *v) { return (v[0] - m[0]) * nrm[0] + (v[1] - m[1]) * nrm[1] + (v[2] - m[2]) * nrm[2]; };
+    int k = 0;
+    const double *prev = in[n - 1];
+    double dp = dist(prev);
+    for (int a = 0; a < n; ++a) {
+        const double *cur = in[a];
+        const double dc = dist(cur);
+        if ((dp < 0.0 && dc > 0.0) || (dp > 0.0 && dc < 0.0)) {
+            if (k == kSurfaceMaxVerts)
+                return -1;
+            const double t = dp / (dp - dc);
+            for (int c = 0; c < 3; ++c)
+                out[k][c] = prev[c] + t * (cur[c] - prev[c]);
+            ++k;
+        }
+        if (dc <= 0.0) {
+            if (k == kSurfaceMaxVerts)
+                return -1;
+            for (int c = 0; c < 3; ++c)
+                out[k][c] = cur[c];
+            ++k;
+        }
+        prev = cur;
+        dp = dc;
+    }
+    return k;
+}
+
+__device__ __forceinline__ void load_point(const float *__restrict__ points, uint32_t i, float *q) {
+    q[0] = __ldg(points + 3 * (uint64_t)i);
+    q[1] = __ldg(points + 3 * (uint64_t)i + 1);
+    q[2] = __ldg(points + 3 * (uint64_t)i + 2);
+}
+
+__device__ __forceinline__ bool same_point(const float *a, const float *b) {
+    return a[0] == b[0] && a[1] == b[1] && a[2] == b[2];
+}
+
+// F_e for entry e of row i into `out` (kSurfaceMaxVerts vertices): its vertex count when the polygon is emitted, 0
+// when it is not (filter, or fewer than 3 vertices), -1 when it needs more than kSurfaceMaxVerts vertices.
+__device__ __forceinline__ int surface_polygon(const SurfaceParams &p, uint32_t i, uint32_t e,
+                                               double (*out)[3]) {
+    const uint32_t j = __ldg(p.adj + e);
+    if (j >= p.num_points || p.inside[j])
+        return 0;
+    float pi[3], pj[3];
+    load_point(p.points, i, pi);
+    load_point(p.points, j, pj);
+    if (same_point(pi, pj))
+        return 0;
+    double buf[kSurfaceMaxVerts][3];
+    double nrm[3], m[3];
+    for (int c = 0; c < 3; ++c) {
+        nrm[c] = (double)pj[c] - (double)pi[c];
+        m[c] = 0.5 * ((double)pi[c] + (double)pj[c]);
+    }
+    // plane ∩ a square around the midpoint that covers the box: half-width twice the box's half-diagonal plus the
+    // midpoint's distance from the box centre, in an orthonormal (u, v) with u x v = nrm / |nrm|
+    double r2 = 0.0, h2 = 0.0;
+    for (int c = 0; c < 3; ++c) {
+        const double lo = p.lo[c], hi = p.hi[c], mid = 0.5 * (lo + hi);
+        r2 += (m[c] - mid) * (m[c] - mid);
+        h2 += 0.25 * (hi - lo) * (hi - lo);
+    }
+    const double R = 2.0 * (sqrt(r2) + sqrt(h2));
+    const double ax = fabs(nrm[0]), ay = fabs(nrm[1]), az = fabs(nrm[2]);
+    const int a = ax <= ay && ax <= az ? 0 : (ay <= az ? 1 : 2); // nrm x (axis of its smallest component)
+    double u[3] = {0.0, 0.0, 0.0};
+    u[(a + 1) % 3] = nrm[(a + 2) % 3];
+    u[(a + 2) % 3] = -nrm[(a + 1) % 3];
+    const double un = sqrt(u[0] * u[0] + u[1] * u[1] + u[2] * u[2]);
+    const double nn = sqrt(nrm[0] * nrm[0] + nrm[1] * nrm[1] + nrm[2] * nrm[2]);
+    for (int c = 0; c < 3; ++c)
+        u[c] /= un;
+    const double v[3] = {(nrm[1] * u[2] - nrm[2] * u[1]) / nn, (nrm[2] * u[0] - nrm[0] * u[2]) / nn,
+                         (nrm[0] * u[1] - nrm[1] * u[0]) / nn};
+    const double su[4] = {1.0, -1.0, -1.0, 1.0}, sv[4] = {1.0, 1.0, -1.0, -1.0};
+    for (int k = 0; k < 4; ++k)
+        for (int c = 0; c < 3; ++c)
+            out[k][c] = m[c] + R * (su[k] * u[c] + sv[k] * v[c]);
+    int n = 4;
+    double(*cur)[3] = out, (*nxt)[3] = buf;
+    auto clip = [&](const double *pn, const double *pm) {
+        n = clip_polygon(cur, n, nxt, pn, pm);
+        double(*t)[3] = cur;
+        cur = nxt;
+        nxt = t;
+    };
+    for (int c = 0; c < 6 && n > 0; ++c) { // the box: x_c <= hi_c, -x_c <= -lo_c
+        double bn[3] = {0.0, 0.0, 0.0}, bm[3] = {0.0, 0.0, 0.0};
+        bn[c % 3] = c < 3 ? 1.0 : -1.0;
+        bm[c % 3] = c < 3 ? p.hi[c % 3] : p.lo[c % 3];
+        clip(bn, bm);
+    }
+    const uint32_t end = min(__ldg(p.off + i + 1), p.num_entries);
+    for (uint32_t k = __ldg(p.off + i); k < end && n > 0; ++k) {
+        const uint32_t q = __ldg(p.adj + k);
+        if (k == e || q >= p.num_points)
+            continue;
+        float pk[3];
+        load_point(p.points, q, pk);
+        if (same_point(pk, pi) || same_point(pk, pj)) // no plane; or plane_e itself, which F_e lies on
+            continue;
+        double kn[3], km[3];
+        for (int c = 0; c < 3; ++c) {
+            kn[c] = (double)pk[c] - (double)pi[c];
+            km[c] = 0.5 * ((double)pi[c] + (double)pk[c]);
+        }
+        clip(kn, km);
+    }
+    if (n < 0)
+        return -1;
+    if (n < 3)
+        return 0;
+    if (cur != out)
+        for (int k = 0; k < n; ++k)
+            for (int c = 0; c < 3; ++c)
+                out[k][c] = cur[k][c];
+    return n;
+}
+
+// Count pass: vcount[e] = vertices of F_e (0 when not emitted), pcount[e] = 1 when emitted; totals[2] counts the
+// polygons that exceeded kSurfaceMaxVerts (they are counted as not emitted).  Every entry of a row in [off[i],
+// min(off[i+1], E)) is written.
+__global__ void __launch_bounds__(kSurfaceBlock) surface_count_kernel(const SurfaceParams p,
+                                                                      unsigned long long *__restrict__ vcount,
+                                                                      uint32_t *__restrict__ pcount,
+                                                                      unsigned long long *__restrict__ totals) {
+    const uint64_t row = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (row >= p.num_points)
+        return;
+    const uint32_t i = (uint32_t)row, lane = threadIdx.x & 31u;
+    const bool in_i = p.inside[i] != 0;
+    const uint32_t end = min(__ldg(p.off + i + 1), p.num_entries);
+    for (uint32_t e = __ldg(p.off + i) + lane; e < end; e += 32) {
+        int n = 0;
+        if (in_i) {
+            double verts[kSurfaceMaxVerts][3];
+            n = surface_polygon(p, i, e, verts);
+        }
+        if (n < 0)
+            atomicAdd(totals + 2, 1ull);
+        vcount[e] = n > 0 ? (unsigned long long)n : 0ull;
+        pcount[e] = n > 0 ? 1u : 0u;
+    }
+}
+
+// Exclusive scan of one (u64, u32) pair per thread over the CTA (warp shuffles, then one warp over the warp
+// totals); *tv / *tc = the CTA's totals.  Ends with a barrier, so the shared state can be reused right away.
+__device__ __forceinline__ void cta_exclusive_scan(unsigned long long &v, uint32_t &c, unsigned long long &tv,
+                                                   uint32_t &tc) {
+    __shared__ unsigned long long warp_v[32];
+    __shared__ uint32_t warp_c[32];
+    __shared__ unsigned long long total_v;
+    __shared__ uint32_t total_c;
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+    unsigned long long iv = v;
+    uint32_t ic = c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long sv = __shfl_up_sync(0xffffffffu, iv, o);
+        const uint32_t sc = __shfl_up_sync(0xffffffffu, ic, o);
+        if ((int)lane >= o) {
+            iv += sv;
+            ic += sc;
+        }
+    }
+    if (lane == 31) {
+        warp_v[warp] = iv;
+        warp_c[warp] = ic;
+    }
+    __syncthreads();
+    if (warp == 0) {
+        const unsigned long long x = lane < nwarps ? warp_v[lane] : 0ull;
+        const uint32_t y = lane < nwarps ? warp_c[lane] : 0u;
+        unsigned long long sx = x;
+        uint32_t sy = y;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long a = __shfl_up_sync(0xffffffffu, sx, o);
+            const uint32_t b = __shfl_up_sync(0xffffffffu, sy, o);
+            if ((int)lane >= o) {
+                sx += a;
+                sy += b;
+            }
+        }
+        if (lane < nwarps) {
+            warp_v[lane] = sx - x;
+            warp_c[lane] = sy - y;
+        }
+        if (lane == 31) {
+            total_v = sx;
+            total_c = sy;
+        }
+    }
+    __syncthreads();
+    v = iv - v + warp_v[warp];
+    c = ic - c + warp_c[warp];
+    tv = total_v;
+    tc = total_c;
+    __syncthreads();
+}
+
+// Scan step 1: per tile of kScanTile entries (kScanItems consecutive ones per thread), the sums.
+__global__ void __launch_bounds__(kScanBlock) scan_tile_sums_kernel(const unsigned long long *__restrict__ v,
+                                                                    const uint32_t *__restrict__ c, uint32_t n,
+                                                                    unsigned long long *__restrict__ tile_v,
+                                                                    uint32_t *__restrict__ tile_c) {
+    const uint64_t base = (uint64_t)blockIdx.x * kScanTile + (uint64_t)threadIdx.x * kScanItems;
+    unsigned long long sv = 0;
+    uint32_t sc = 0;
+    for (int k = 0; k < kScanItems; ++k)
+        if (base + k < n) {
+            sv += v[base + k];
+            sc += c[base + k];
+        }
+    unsigned long long tv;
+    uint32_t tc;
+    cta_exclusive_scan(sv, sc, tv, tc);
+    if (threadIdx.x == 0) {
+        tile_v[blockIdx.x] = tv;
+        tile_c[blockIdx.x] = tc;
+    }
+}
+
+// Scan step 2 (one CTA): the tile sums become exclusive tile prefixes; the grand totals go to v[n], c[n] and
+// totals[0..1].
+__global__ void __launch_bounds__(kScanBlock) scan_tile_prefix_kernel(unsigned long long *__restrict__ tile_v,
+                                                                      uint32_t *__restrict__ tile_c, uint32_t tiles,
+                                                                      unsigned long long *__restrict__ v,
+                                                                      uint32_t *__restrict__ c, uint32_t n,
+                                                                      unsigned long long *__restrict__ totals) {
+    unsigned long long carry_v = 0;
+    uint32_t carry_c = 0;
+    for (uint32_t t0 = 0; t0 < tiles; t0 += kScanBlock) {
+        const uint32_t t = t0 + threadIdx.x;
+        unsigned long long x = t < tiles ? tile_v[t] : 0ull;
+        uint32_t y = t < tiles ? tile_c[t] : 0u;
+        unsigned long long tv;
+        uint32_t tc;
+        cta_exclusive_scan(x, y, tv, tc);
+        if (t < tiles) {
+            tile_v[t] = carry_v + x;
+            tile_c[t] = carry_c + y;
+        }
+        carry_v += tv;
+        carry_c += tc;
+    }
+    if (threadIdx.x == 0) {
+        v[n] = carry_v;
+        c[n] = carry_c;
+        totals[0] = carry_v;
+        totals[1] = carry_c;
+    }
+}
+
+// Scan step 3: each tile's exclusive scan plus its tile prefix, in place.
+__global__ void __launch_bounds__(kScanBlock) scan_add_back_kernel(unsigned long long *__restrict__ v,
+                                                                   uint32_t *__restrict__ c, uint32_t n,
+                                                                   const unsigned long long *__restrict__ tile_v,
+                                                                   const uint32_t *__restrict__ tile_c) {
+    const uint64_t base = (uint64_t)blockIdx.x * kScanTile + (uint64_t)threadIdx.x * kScanItems;
+    unsigned long long xv[kScanItems], sv = 0;
+    uint32_t xc[kScanItems], sc = 0;
+    for (int k = 0; k < kScanItems; ++k) {
+        const bool ok = base + k < n;
+        xv[k] = ok ? v[base + k] : 0ull;
+        xc[k] = ok ? c[base + k] : 0u;
+        sv += xv[k];
+        sc += xc[k];
+    }
+    unsigned long long tv;
+    uint32_t tc;
+    cta_exclusive_scan(sv, sc, tv, tc);
+    sv += tile_v[blockIdx.x];
+    sc += tile_c[blockIdx.x];
+    for (int k = 0; k < kScanItems; ++k)
+        if (base + k < n) {
+            v[base + k] = sv;
+            c[base + k] = sc;
+            sv += xv[k];
+            sc += xc[k];
+        }
+}
+
+// Write pass: the polygon of entry e goes to vertices [voff[e], voff[e+1]) and polygon slot poff[e] -- only when the
+// count pass emitted it (poff[e+1] - poff[e] == 1) and it has exactly the counted vertex run, so nothing is ever
+// written outside the counted output.  rgb = the colour of cell i along normalize(p_i - p_j), computed as
+// sample_field_kernel computes it for that direction.
+template <int DEG, typename AttrT>
+__global__ void __launch_bounds__(kSurfaceBlock) surface_write_kernel(
+    const SurfaceParams p, const AttrT *__restrict__ attrs, const unsigned long long *__restrict__ voff,
+    const uint32_t *__restrict__ poff, const unsigned long long *__restrict__ totals, float *__restrict__ vertices,
+    long long *__restrict__ offsets, uint32_t *__restrict__ cells, AttrT *__restrict__ rgb) {
+    constexpr int A = attr_dim(DEG), NC = 3 * sh_dim(DEG);
+    const uint64_t row = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (row == 0 && threadIdx.x == 0)
+        offsets[totals[1]] = (long long)totals[0];
+    if (row >= p.num_points)
+        return;
+    const uint32_t i = (uint32_t)row, lane = threadIdx.x & 31u;
+    if (!p.inside[i])
+        return;
+    const uint32_t end = min(__ldg(p.off + i + 1), p.num_entries);
+    for (uint32_t e = __ldg(p.off + i) + lane; e < end; e += 32) {
+        const uint32_t slot = poff[e];
+        if (poff[e + 1] - slot != 1u)
+            continue;
+        const unsigned long long v0 = voff[e], count = voff[e + 1] - v0;
+        double verts[kSurfaceMaxVerts][3];
+        const int n = surface_polygon(p, i, e, verts);
+        if (n <= 0 || (unsigned long long)n != count)
+            continue;
+        for (int k = 0; k < n; ++k)
+            for (int c = 0; c < 3; ++c)
+                vertices[3 * (v0 + k) + c] = __double2float_rn(verts[k][c]);
+        const uint32_t j = __ldg(p.adj + e);
+        offsets[slot] = (long long)v0;
+        cells[2 * (uint64_t)slot] = i;
+        cells[2 * (uint64_t)slot + 1] = j;
+        float pi[3], pj[3];
+        load_point(p.points, i, pi);
+        load_point(p.points, j, pj);
+        float dx = __fsub_rn(pi[0], pj[0]), dy = __fsub_rn(pi[1], pj[1]), dz = __fsub_rn(pi[2], pj[2]);
+        normalize_dir(dx, dy, dz);
+        float sh[sh_dim(DEG)];
+        sh_basis<DEG>(dx, dy, dz, sh);
+        const AttrT *arow = attrs + (uint64_t)i * A;
+        float cv[NC];
+#pragma unroll
+        for (int k = 0; k < NC; ++k)
+            cv[k] = (float)arow[k];
+        float r, g, b;
+        sh_coeffs_to_rgb<DEG>(cv, sh, r, g, b);
+        rgb[3 * (uint64_t)slot] = (AttrT)r;
+        rgb[3 * (uint64_t)slot + 1] = (AttrT)g;
+        rgb[3 * (uint64_t)slot + 2] = (AttrT)b;
+    }
+}
+
 } // namespace rfb

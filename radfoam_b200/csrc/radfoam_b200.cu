@@ -5,6 +5,7 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <mutex>
@@ -1012,6 +1013,123 @@ int rfb_sample_field_backward(rfb_pipeline *p, uint32_t num_points, uint32_t num
     if (half)
         cudaFreeAsync(acc, stream); // stream-ordered: after the kernels above, also on the error path
     RFB_CUDA(launched);
+    return 0;
+}
+
+} // extern "C"
+
+namespace {
+// Layout of the surface scratch: totals (4 u64), vertex offsets (E+1 u64), tile sums (u64), polygon offsets
+// (E+1 u32), tile sums (u32).
+struct SurfaceScratch {
+    unsigned long long *totals, *voff, *tile_v;
+    uint32_t *poff, *tile_c;
+    uint32_t tiles;
+};
+
+uint64_t surface_scratch(uint32_t num_entries, void *base, SurfaceScratch *s) {
+    const uint64_t tiles = ((uint64_t)num_entries + kScanTile - 1) / kScanTile;
+    const uint64_t n64 = 4 + (uint64_t)num_entries + 1 + tiles, n32 = (uint64_t)num_entries + 1 + tiles;
+    if (s) {
+        char *b = static_cast<char *>(base);
+        s->totals = reinterpret_cast<unsigned long long *>(b);
+        s->voff = s->totals + 4;
+        s->tile_v = s->voff + num_entries + 1;
+        s->poff = reinterpret_cast<uint32_t *>(s->tile_v + tiles);
+        s->tile_c = s->poff + num_entries + 1;
+        s->tiles = (uint32_t)tiles;
+    }
+    return 8 * n64 + 4 * n32;
+}
+
+int surface_params(const char *who, const float *points, uint32_t num_points, uint32_t num_entries,
+                   const uint32_t *adj, const uint32_t *off, const uint8_t *inside, const rfb_box *bounds,
+                   const void *scratch, SurfaceParams *sp) {
+    if (!points || !off || !inside || !bounds || !scratch || (num_entries && !adj))
+        return fail(std::string(who) + ": NULL argument");
+    for (int c = 0; c < 3; ++c)
+        if (!(bounds->lo[c] <= bounds->hi[c]) || !std::isfinite(bounds->lo[c]) || !std::isfinite(bounds->hi[c]))
+            return fail(std::string(who) + ": bounds must be finite with lo <= hi");
+    sp->points = points;
+    sp->adj = adj;
+    sp->off = off;
+    sp->inside = inside;
+    sp->num_points = num_points;
+    sp->num_entries = num_entries;
+    for (int c = 0; c < 3; ++c) {
+        sp->lo[c] = bounds->lo[c];
+        sp->hi[c] = bounds->hi[c];
+    }
+    return 0;
+}
+} // namespace
+
+extern "C" {
+
+uint64_t rfb_surface_scratch_bytes(uint32_t point_adjacency_size) {
+    return surface_scratch(point_adjacency_size, nullptr, nullptr);
+}
+
+int rfb_surface_count(const float *points, uint32_t num_points, uint32_t point_adjacency_size,
+                      const uint32_t *point_adjacency, const uint32_t *point_adjacency_offsets, const uint8_t *inside,
+                      const rfb_box *bounds, void *scratch, void *stream_) {
+    SurfaceParams sp;
+    if (int rc = surface_params("rfb_surface_count", points, num_points, point_adjacency_size, point_adjacency,
+                                point_adjacency_offsets, inside, bounds, scratch, &sp))
+        return rc;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    SurfaceScratch s;
+    surface_scratch(point_adjacency_size, scratch, &s);
+    RFB_CUDA(cudaMemsetAsync(s.totals, 0, 4 * sizeof(unsigned long long), stream));
+    if (num_points) {
+        RFB_LAUNCH((surface_count_kernel), (uint32_t)(((uint64_t)num_points * 32 + kSurfaceBlock - 1) / kSurfaceBlock),
+                   kSurfaceBlock, 0, stream, sp, s.voff, s.poff, s.totals);
+        ++g_launches;
+    }
+    if (s.tiles) {
+        RFB_LAUNCH((scan_tile_sums_kernel), s.tiles, kScanBlock, 0, stream, s.voff, s.poff, point_adjacency_size,
+                   s.tile_v, s.tile_c);
+        ++g_launches;
+    }
+    RFB_LAUNCH((scan_tile_prefix_kernel), 1, kScanBlock, 0, stream, s.tile_v, s.tile_c, s.tiles, s.voff, s.poff,
+               point_adjacency_size, s.totals);
+    ++g_launches;
+    if (s.tiles) {
+        RFB_LAUNCH((scan_add_back_kernel), s.tiles, kScanBlock, 0, stream, s.voff, s.poff, point_adjacency_size,
+                   s.tile_v, s.tile_c);
+        ++g_launches;
+    }
+    RFB_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int rfb_surface_write(rfb_pipeline *p, const float *points, uint32_t num_points, const void *attributes,
+                      uint32_t point_adjacency_size, const uint32_t *point_adjacency,
+                      const uint32_t *point_adjacency_offsets, const uint8_t *inside, const rfb_box *bounds,
+                      const void *scratch, float *vertices, int64_t *offsets, uint32_t *cells, void *rgb,
+                      void *stream_) {
+    if (!p)
+        return fail("rfb_surface_write: pipeline is NULL");
+    SurfaceParams sp;
+    if (int rc = surface_params("rfb_surface_write", points, num_points, point_adjacency_size, point_adjacency,
+                                point_adjacency_offsets, inside, bounds, scratch, &sp))
+        return rc;
+    // vertices / cells / rgb are written only for counted polygons: they may be NULL when the count found none
+    if (!offsets || (num_points && !attributes))
+        return fail("rfb_surface_write: NULL argument");
+    cudaStream_t stream = (cudaStream_t)stream_;
+    SurfaceScratch s;
+    surface_scratch(point_adjacency_size, const_cast<void *>(scratch), &s);
+    const uint32_t grid = (uint32_t)(((uint64_t)(num_points ? num_points : 1) * 32 + kSurfaceBlock - 1) / kSurfaceBlock);
+    with_degree(p->sh_degree, [&](auto d) {
+        with_attr_type(p->attr_dtype, [&](auto t) {
+            using AttrT = typename decltype(t)::type;
+            RFB_LAUNCH((surface_write_kernel<decltype(d)::value, AttrT>), grid, kSurfaceBlock, 0, stream, sp,
+                       reinterpret_cast<const AttrT *>(attributes), s.voff, s.poff, s.totals, vertices,
+                       reinterpret_cast<long long *>(offsets), cells, reinterpret_cast<AttrT *>(rgb));
+        });
+    });
+    RFB_LAUNCHED();
     return 0;
 }
 

@@ -860,6 +860,84 @@ class Pipeline:
                 _ptr(attr_grad), stream))
         return attr_grad
 
+    # ---- the density surface as Voronoi faces (rfb_surface_count / rfb_surface_write): not part of the reference
+    def extract_surface(self, points, attributes, point_adjacency, point_adjacency_offsets, threshold=None,
+                        inside=None, bounds=None):
+        """The boundary between occupied and empty cells, as the exact Voronoi faces between them.
+
+        Occupied cells are ``attributes[:, -1] > threshold`` or the bool ``[N]`` mask ``inside`` (pass exactly one).
+        Every CSR entry ``(i, j)`` with ``i`` occupied, ``j`` empty and ``p_j != p_i`` gives the polygon where cell
+        ``i`` -- clipped to ``bounds`` and to the bisector planes of its listed neighbours, the region the walk treats
+        as cell ``i`` -- meets the bisector plane of ``(i, j)``, when it has at least 3 vertices.  Polygons come in
+        CSR order, counter-clockwise seen from ``j`` (normals point out of the occupied cells), computed in float64
+        and rounded once to float32; nothing is welded.  ``bounds = (lo[3], hi[3])`` defaults to the points'
+        bounding box; the surface is open where occupied cells reach it.
+
+        Returns ``{"vertices" f32[V, 3], "offsets" int64[P+1], "cells" uint32[P, 2], "rgb" [P, 3],
+        "triangles" int64[V-2P, 3]}``: polygon ``k`` is ``vertices[offsets[k]:offsets[k+1]]`` between cells
+        ``cells[k] = (i, j)``; ``rgb`` (attribute dtype) is cell ``i``'s colour along ``normalize(p_i - p_j)``, as
+        :meth:`sample_field` gives it; ``triangles`` fan each polygon from its first vertex.
+
+        The output sizes are read back from the device once (and, without ``bounds``, the bounding box), so the call
+        synchronises with the current stream and cannot be captured in a CUDA graph.  Raises when a polygon needs more
+        vertices than the kernels hold (32)."""
+        self._validate_scene(points, attributes, point_adjacency, point_adjacency_offsets)
+        if attributes is None:
+            raise RuntimeError("extract_surface needs the attributes (a bound parameter-form scene is not used here)")
+        if (threshold is None) == (inside is None):
+            raise RuntimeError("extract_surface: pass exactly one of threshold and inside")
+        pts, attrs = points.detach().contiguous(), attributes.detach().contiguous()
+        if pts.dim() != 2:
+            raise RuntimeError("points must have shape [N, 3]")
+        adj, off = point_adjacency.contiguous(), point_adjacency_offsets.contiguous()
+        dev, n = pts.device, pts.size(0)
+        if adj.device != dev or off.device != dev or attrs.device != dev:
+            raise RuntimeError("extract_surface: every tensor must be on the points' device")
+        if inside is None:
+            occupied = (attrs[:, -1] > float(threshold)).contiguous()
+        else:
+            if not isinstance(inside, torch.Tensor) or inside.dtype != torch.bool or inside.device != dev \
+                    or tuple(inside.shape) != (n,):
+                raise RuntimeError("inside must be a bool tensor [N] on the points' device")
+            occupied = inside.detach().contiguous()
+        box = _lib.Box()
+        if bounds is None:
+            if n:
+                lo, hi = torch.stack([pts.amin(0), pts.amax(0)]).cpu().tolist()
+            else:
+                lo, hi = [0.0] * 3, [0.0] * 3
+        else:
+            lo, hi = (torch.as_tensor(b, dtype=torch.float32).detach().cpu().reshape(-1).tolist() for b in bounds)
+            if len(lo) != 3 or len(hi) != 3:
+                raise RuntimeError("bounds must be (lo[3], hi[3])")
+        box.lo[:], box.hi[:] = lo, hi
+        e = adj.numel()
+        scratch = torch.empty((int(self._lib.rfb_surface_scratch_bytes(e)) + 7) // 8, dtype=torch.int64, device=dev)
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            _lib.check(self._lib.rfb_surface_count(
+                _ptr(pts), n, e, _ptr(adj) if e else None, _ptr(off), _ptr(occupied), ctypes.byref(box),
+                _ptr(scratch), stream))
+            nv, npoly, over = (int(x) for x in scratch[:3].cpu().tolist())
+            if over:
+                raise RuntimeError(f"extract_surface: {over} polygons need more than 32 vertices; "
+                                   "no surface was written")
+            vertices = torch.empty((nv, 3), dtype=torch.float32, device=dev)
+            offsets = torch.empty((npoly + 1,), dtype=torch.int64, device=dev)
+            cells = torch.empty((npoly, 2), dtype=torch.uint32, device=dev)
+            rgb = torch.empty((npoly, 3), dtype=self._dtype, device=dev)
+            _lib.check(self._lib.rfb_surface_write(
+                self._handle, _ptr(pts), n, _ptr(attrs), e, _ptr(adj) if e else None, _ptr(off), _ptr(occupied),
+                ctypes.byref(box), _ptr(scratch), _ptr(vertices), _ptr(offsets), _ptr(cells), _ptr(rgb), stream))
+        # fan triangulation: polygon k gives (o_k, o_k + t + 1, o_k + t + 2) for t < count_k - 2
+        fan = torch.diff(offsets) - 2
+        ntri = nv - 2 * npoly
+        first = torch.repeat_interleave(offsets[:-1], fan, output_size=ntri)
+        start = torch.repeat_interleave(torch.cumsum(fan, 0) - fan, fan, output_size=ntri)
+        t = torch.arange(ntri, device=dev) - start
+        triangles = torch.stack([first, first + t + 1, first + t + 2], -1)
+        return {"vertices": vertices, "offsets": offsets, "cells": cells, "rgb": rgb, "triangles": triangles}
+
     # radfoam::prefetch_adjacent_diff (pipeline.h:50-56); handy for trace_benchmark callers
     def prefetch_adjacent_diff(self, points, point_adjacency, point_adjacency_offsets):
         points_c = points.contiguous()

@@ -150,6 +150,48 @@ class FoamScene:
                    activation_scale=activation_scale)
 
 
+def save_surface_ply(path, surface) -> None:
+    """Write a ``Pipeline.extract_surface`` result as a binary little-endian PLY mesh: one vertex element (``x y z``
+    float, ``red green blue`` uchar: each vertex takes its polygon's colour, clamped to [0, 1] and truncated from
+    ``x 255`` in float32 as the tracer's RGBA8 packing does) and one face element (``vertex_indices``: a uchar count
+    and int indices).  Polygons are written as they are -- shared vertices are not welded.  The mesh counterpart of
+    the reference's point-cloud ``save_ply`` (radfoam_model/scene.py:550-612)."""
+    import numpy as np
+
+    def host(t):
+        return t.detach().cpu().numpy() if isinstance(t, torch.Tensor) else np.asarray(t)
+
+    vertices = np.ascontiguousarray(host(surface["vertices"]), dtype=np.float32).reshape(-1, 3)
+    offsets = host(surface["offsets"]).astype(np.int64).reshape(-1)
+    rgb = host(surface["rgb"]).astype(np.float32).reshape(-1, 3)
+    nv, npoly = vertices.shape[0], offsets.shape[0] - 1
+    counts = np.diff(offsets)
+    if npoly < 0 or rgb.shape[0] != npoly or offsets[0] != 0 or offsets[-1] != nv or (counts < 3).any() \
+            or (counts > 255).any() or nv >= 2 ** 31:
+        raise ValueError("not a surface: offsets[P+1] must partition the vertices into polygons of 3..255 vertices, "
+                         "with one rgb row per polygon")
+    # fmax(0, fmin(1, c)) maps NaN to 1, like fmaxf(0, fminf(1, c)) in the kernels
+    colour = (np.fmax(np.float32(0), np.fmin(np.float32(1), rgb)) * np.float32(255)).astype(np.uint8)
+    vrec = np.empty(nv, dtype=[("x", "<f4"), ("y", "<f4"), ("z", "<f4"),
+                               ("red", "u1"), ("green", "u1"), ("blue", "u1")])
+    vrec["x"], vrec["y"], vrec["z"] = vertices[:, 0], vertices[:, 1], vertices[:, 2]
+    per_vertex = np.repeat(colour, counts, axis=0)
+    vrec["red"], vrec["green"], vrec["blue"] = per_vertex[:, 0], per_vertex[:, 1], per_vertex[:, 2]
+    # face k = [count_k][int32 indices offsets[k] .. offsets[k+1]-1]; it starts at byte k + 4 offsets[k]
+    faces = np.empty(npoly + 4 * nv, dtype=np.uint8)
+    faces[np.arange(npoly) + 4 * offsets[:-1]] = counts.astype(np.uint8)
+    at = np.repeat(np.arange(npoly, dtype=np.int64), counts) + 1 + 4 * np.arange(nv, dtype=np.int64)
+    faces[at[:, None] + np.arange(4)] = np.arange(nv, dtype="<i4").view(np.uint8).reshape(nv, 4)
+    header = ("ply\nformat binary_little_endian 1.0\n"
+              f"element vertex {nv}\nproperty float x\nproperty float y\nproperty float z\n"
+              "property uchar red\nproperty uchar green\nproperty uchar blue\n"
+              f"element face {npoly}\nproperty list uchar int vertex_indices\nend_header\n")
+    with open(path, "wb") as f:
+        f.write(header.encode("ascii"))
+        f.write(vrec.tobytes())
+        f.write(faces.tobytes())
+
+
 def _to_uint32(t):
     if t.numel() and (int(t.min()) < 0 or int(t.max()) > 0xFFFFFFFF):
         raise RuntimeError("adjacency values do not fit uint32")
