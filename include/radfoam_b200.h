@@ -15,6 +15,7 @@
  *   rfb_locate_points        <- radfoam::nn over the AABB tree  src/aabb_tree/aabb_tree.cu:343-415 (any number of queries)
  *   rfb_sample_field(_backward)  (new) the field at arbitrary points and its attribute gradient
  *   rfb_surface_count/_write     (new) the Voronoi faces between occupied and empty cells, as polygons
+ *   rfb_delaunay_count/_write    <- radfoam::Triangulation::point_adjacency  src/delaunay/delaunay.h (by Voronoi clipping)
  *
  * The reference interface is a C++ vtable taking raw device pointers (Eigen
  * types appear only as reinterpret_casts of packed floats); this header
@@ -260,6 +261,32 @@ int rfb_surface_write(rfb_pipeline *pipeline, const float *points, uint32_t num_
                       const uint32_t *point_adjacency_offsets, const uint8_t *inside, const rfb_box *bounds,
                       const void *scratch, float *vertices, int64_t *offsets, uint32_t *cells, void *rgb,
                       void *stream);
+
+/* ---- Delaunay adjacency: the point graph the tracer walks, built on the GPU ----
+ * Definition.  For a closed box B containing the points, {i, j} (i != j) is an edge iff the face
+ *   F_ij = { x in B : |x - p_i| = |x - p_j| <= |x - p_k| for all k }
+ * has positive area (points read as their exact float64 values).  For points in general position this is the
+ * Delaunay graph minus the edges whose Voronoi face lies wholly outside B.  Faces of zero area (co-spherical ties,
+ * e.g. lattice diagonals) may be present or absent, but always from both ends.  Output: CSR rows strictly ascending,
+ * no self entries, symmetric; two builds of the same input give identical bytes.
+ * `order` must be a permutation of 0..N-1 listing the points in a spatially coherent order (a Morton order); it
+ * affects the speed only.  Two equal points, a non-finite coordinate or an `order` that is not a permutation fail the
+ * build (reported in the totals); nothing is then written out of range, but the graph is unspecified.
+ *
+ * Two passes, both allocation-free:
+ *   rfb_delaunay_count  fills `scratch` (rfb_delaunay_scratch_bytes(N, pool_capacity) bytes of device memory, any
+ *     contents).  It starts with uint64 totals[8] = {entries found from one end only, edges E, face entries needed
+ *     in the pool, cells finished by the overflow kernel, duplicate points, non-finite points, cells over the
+ *     overflow kernel's capacity, bad `order` entries}.  When totals[2] > pool_capacity the count must be repeated
+ *     with a larger pool; when totals[4..7] are not all 0 the build failed.
+ *   rfb_delaunay_write  (same N, order and pool_capacity, the scratch of a successful count) writes
+ *     point_adjacency[E] and point_adjacency_offsets[N+1], using `rows` (E uint32 of device memory) as work space.
+ *     Sizing the outputs needs totals[1] on the host: a caller synchronises between the two. */
+uint64_t rfb_delaunay_scratch_bytes(uint32_t num_points, uint32_t pool_capacity);
+int rfb_delaunay_count(const float *points, uint32_t num_points, const uint32_t *order, const rfb_box *bounds,
+                       uint32_t pool_capacity, void *scratch, void *stream);
+int rfb_delaunay_write(uint32_t num_points, const uint32_t *order, uint32_t pool_capacity, const void *scratch,
+                       uint32_t *rows, uint32_t *point_adjacency, uint32_t *point_adjacency_offsets, void *stream);
 
 int rfb_trace_forward(rfb_pipeline *pipeline, const rfb_trace_settings *settings,
                       uint32_t num_points, const float *points,

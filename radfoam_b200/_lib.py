@@ -81,6 +81,9 @@ SIGNATURES = {
     "rfb_surface_count": (c_int, [_P, c_uint32, c_uint32, _P, _P, _P, POINTER(Box), _P, _P]),
     "rfb_surface_write": (c_int, [_P, _P, c_uint32, _P, c_uint32, _P, _P, _P, POINTER(Box), _P, _P, _P, _P, _P,
                                   _P]),
+    "rfb_delaunay_scratch_bytes": (c_uint64, [c_uint32, c_uint32]),
+    "rfb_delaunay_count": (c_int, [_P, c_uint32, _P, POINTER(Box), c_uint32, _P, _P]),
+    "rfb_delaunay_write": (c_int, [c_uint32, _P, c_uint32, _P, _P, _P, _P, _P]),
     "rfb_trace_forward": (c_int, [_P, POINTER(TraceSettings), c_uint32, _P, _P, c_uint32, _P, _P,
                                   c_uint32, _P, _P, c_uint32, _P, _P, _P, _P, _P, _P,
                                   POINTER(LaunchOpts), _P]),

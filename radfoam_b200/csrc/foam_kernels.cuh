@@ -1955,7 +1955,8 @@ struct SurfaceParams {
 
 // Keeps the part of `in` (n vertices) where (x - m).nrm <= 0, vertex order preserved (Sutherland-Hodgman).  A new
 // vertex is made only where an edge crosses the plane strictly, so a vertex on the plane is never doubled.  Returns
-// the vertex count, or -1 when it would exceed kSurfaceMaxVerts.  NaN distances drop their vertices.
+// the vertex count, or -1 when it would exceed MaxVerts.  NaN distances drop their vertices.
+template <int MaxVerts = kSurfaceMaxVerts>
 __device__ __forceinline__ int clip_polygon(const double (*in)[3], int n, double (*out)[3], const double *nrm,
                                             const double *m) {
     if (n == 0)
@@ -1968,7 +1969,7 @@ __device__ __forceinline__ int clip_polygon(const double (*in)[3], int n, double
         const double *cur = in[a];
         const double dc = dist(cur);
         if ((dp < 0.0 && dc > 0.0) || (dp > 0.0 && dc < 0.0)) {
-            if (k == kSurfaceMaxVerts)
+            if (k == MaxVerts)
                 return -1;
             const double t = dp / (dp - dc);
             for (int c = 0; c < 3; ++c)
@@ -1976,7 +1977,7 @@ __device__ __forceinline__ int clip_polygon(const double (*in)[3], int n, double
             ++k;
         }
         if (dc <= 0.0) {
-            if (k == kSurfaceMaxVerts)
+            if (k == MaxVerts)
                 return -1;
             for (int c = 0; c < 3; ++c)
                 out[k][c] = cur[c];

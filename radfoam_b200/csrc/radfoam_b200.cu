@@ -16,6 +16,7 @@
 #include <type_traits>
 
 #include "foam_kernels.cuh"
+#include "delaunay_kernels.cuh"
 
 // Kernel launch.  In the product this is the <<< >>> launch; the CPU kernel-logic emulator under tests/emu
 // (test infrastructure, never loaded by the product) defines RFB_LAUNCH itself before this file is compiled.
@@ -1130,6 +1131,158 @@ int rfb_surface_write(rfb_pipeline *p, const float *points, uint32_t num_points,
         });
     });
     RFB_LAUNCHED();
+    return 0;
+}
+
+} // extern "C"
+
+namespace {
+// Layout of the Delaunay scratch, every piece 256-byte aligned: totals (8 u64), scan values v (N+1 u64) and their
+// tile sums, row sizes c (N+1 u32, the offsets after the scan) and their tile sums, per sorted cell start / count /
+// extra / cursor (u32), the overflow list (u32), the sorted points, the tree, the face pool and the overflow slices.
+struct DelaunayScratch {
+    unsigned long long *totals, *v, *tile_v;
+    uint32_t *c, *tile_c, *start, *count, *extra, *cursor, *overflow, *pool;
+    float *sorted, *tree;
+    char *slices;
+    uint32_t tiles, pow2;
+};
+
+// Overflow warps (and scratch slices): one per kDelOvfPointsPerWarp points, at most kDelOvfWarps.
+uint32_t delaunay_overflow_warps(uint32_t n) {
+    const uint64_t w = ((uint64_t)n + kDelOvfPointsPerWarp - 1) / kDelOvfPointsPerWarp;
+    return (uint32_t)(w < 1 ? 1 : (w > (uint64_t)kDelOvfWarps ? kDelOvfWarps : w));
+}
+
+uint64_t delaunay_scratch(uint32_t n, uint32_t pool_capacity, void *base, DelaunayScratch *s) {
+    const uint64_t tiles = ((uint64_t)n + kScanTile - 1) / kScanTile;
+    uint64_t leaves = ((uint64_t)n + kDelLeaf - 1) / kDelLeaf, pow2 = 1;
+    while (pow2 < leaves)
+        pow2 *= 2;
+    uint64_t at = 0;
+    char *b = static_cast<char *>(base);
+    auto take = [&](uint64_t bytes) {
+        char *p = b ? b + at : nullptr;
+        at += (bytes + 255) / 256 * 256;
+        return p;
+    };
+    char *totals = take(8 * kDelTotals), *v = take(8 * ((uint64_t)n + 1)), *tile_v = take(8 * tiles);
+    char *c = take(4 * ((uint64_t)n + 1)), *tile_c = take(4 * tiles);
+    char *start = take(4 * (uint64_t)n), *count = take(4 * (uint64_t)n), *extra = take(4 * (uint64_t)n);
+    char *cursor = take(4 * (uint64_t)n), *overflow = take(4 * (uint64_t)n);
+    char *sorted = take(12 * (uint64_t)n), *tree = take(24 * 2 * pow2), *pool = take(4 * (uint64_t)pool_capacity);
+    char *slices = take(kDelOvfSliceBytes * delaunay_overflow_warps(n));
+    if (s) {
+        s->totals = reinterpret_cast<unsigned long long *>(totals);
+        s->v = reinterpret_cast<unsigned long long *>(v);
+        s->tile_v = reinterpret_cast<unsigned long long *>(tile_v);
+        s->c = reinterpret_cast<uint32_t *>(c);
+        s->tile_c = reinterpret_cast<uint32_t *>(tile_c);
+        s->start = reinterpret_cast<uint32_t *>(start);
+        s->count = reinterpret_cast<uint32_t *>(count);
+        s->extra = reinterpret_cast<uint32_t *>(extra);
+        s->cursor = reinterpret_cast<uint32_t *>(cursor);
+        s->overflow = reinterpret_cast<uint32_t *>(overflow);
+        s->pool = reinterpret_cast<uint32_t *>(pool);
+        s->sorted = reinterpret_cast<float *>(sorted);
+        s->tree = reinterpret_cast<float *>(tree);
+        s->slices = slices;
+        s->tiles = (uint32_t)tiles;
+        s->pow2 = (uint32_t)pow2;
+    }
+    return at;
+}
+
+uint32_t blocks_for(uint64_t items, int block) { return (uint32_t)((items + block - 1) / block); }
+} // namespace
+
+extern "C" {
+
+uint64_t rfb_delaunay_scratch_bytes(uint32_t num_points, uint32_t pool_capacity) {
+    return delaunay_scratch(num_points, pool_capacity, nullptr, nullptr);
+}
+
+int rfb_delaunay_count(const float *points, uint32_t num_points, const uint32_t *order, const rfb_box *bounds,
+                       uint32_t pool_capacity, void *scratch, void *stream_) {
+    if (!scratch || !bounds || (num_points && (!points || !order)))
+        return fail("rfb_delaunay_count: NULL argument");
+    if (num_points >= (1u << 31))
+        return fail("rfb_delaunay_count: at most 2^31 - 1 points");
+    for (int c = 0; c < 3; ++c)
+        if (!(bounds->lo[c] <= bounds->hi[c]) || !std::isfinite(bounds->lo[c]) || !std::isfinite(bounds->hi[c]))
+            return fail("rfb_delaunay_count: bounds must be finite with lo <= hi");
+    cudaStream_t stream = (cudaStream_t)stream_;
+    DelaunayScratch s;
+    delaunay_scratch(num_points, pool_capacity, scratch, &s);
+    const uint32_t n = num_points;
+    RFB_CUDA(cudaMemsetAsync(s.totals, 0, 8 * kDelTotals, stream));
+    if (n) {
+        RFB_CUDA(cudaMemsetAsync(s.extra, 0, 4 * (uint64_t)n, stream));
+        RFB_CUDA(cudaMemsetAsync(s.cursor, 0, 4 * (uint64_t)n, stream)); // the gather's permutation check
+        RFB_CUDA(cudaMemsetAsync(s.v, 0, 8 * ((uint64_t)n + 1), stream));
+        RFB_CUDA(cudaMemsetAsync(s.c, 0, 4 * ((uint64_t)n + 1), stream));
+        DelaunayParams P;
+        P.points = s.sorted;
+        P.tree = s.tree;
+        P.n = n;
+        P.pow2 = s.pow2;
+        for (int c = 0; c < 3; ++c) {
+            P.lo[c] = bounds->lo[c];
+            P.hi[c] = bounds->hi[c];
+        }
+        RFB_LAUNCH((delaunay_gather_kernel), blocks_for(n, kDelBlock), kDelBlock, 0, stream, points, order, n, s.sorted,
+                   s.cursor, s.totals);
+        RFB_LAUNCH((delaunay_leaf_kernel), blocks_for(s.pow2, kDelBlock), kDelBlock, 0, stream, s.sorted, n, s.pow2,
+                   s.tree);
+        g_launches += 2;
+        for (uint32_t first = s.pow2 / 2; first >= 1; first /= 2) {
+            RFB_LAUNCH((delaunay_level_kernel), blocks_for(first, kDelBlock), kDelBlock, 0, stream, first, s.tree);
+            ++g_launches;
+        }
+        RFB_LAUNCH((delaunay_clip_kernel), blocks_for(n, kDelBlock), kDelBlock, 0, stream, P, s.pool, pool_capacity,
+                   s.start, s.count, s.overflow, s.totals);
+        RFB_LAUNCH((delaunay_overflow_kernel), delaunay_overflow_warps(n), 32, 0, stream, P, s.overflow,
+                   s.slices, s.pool, pool_capacity, s.start, s.count, s.totals);
+        RFB_LAUNCH((delaunay_extra_kernel), blocks_for(n, kDelBlock), kDelBlock, 0, stream, n, s.pool, s.start,
+                   s.count, s.extra);
+        RFB_LAUNCH((delaunay_count_kernel), blocks_for(n, kDelBlock), kDelBlock, 0, stream, n, order, s.start, s.count,
+                   s.extra, s.v, s.c);
+        g_launches += 4;
+    }
+    if (s.tiles) {
+        RFB_LAUNCH((scan_tile_sums_kernel), s.tiles, kScanBlock, 0, stream, s.v, s.c, n, s.tile_v, s.tile_c);
+        ++g_launches;
+    }
+    RFB_LAUNCH((scan_tile_prefix_kernel), 1, kScanBlock, 0, stream, s.tile_v, s.tile_c, s.tiles, s.v, s.c, n,
+               s.totals);
+    ++g_launches;
+    if (s.tiles) {
+        RFB_LAUNCH((scan_add_back_kernel), s.tiles, kScanBlock, 0, stream, s.v, s.c, n, s.tile_v, s.tile_c);
+        ++g_launches;
+    }
+    RFB_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int rfb_delaunay_write(uint32_t num_points, const uint32_t *order, uint32_t pool_capacity, const void *scratch,
+                       uint32_t *rows, uint32_t *point_adjacency, uint32_t *point_adjacency_offsets, void *stream_) {
+    // rows and point_adjacency are written only for counted edges: they may be NULL when the count found none
+    if (!scratch || !point_adjacency_offsets || (num_points && !order))
+        return fail("rfb_delaunay_write: NULL argument");
+    cudaStream_t stream = (cudaStream_t)stream_;
+    DelaunayScratch s;
+    delaunay_scratch(num_points, pool_capacity, const_cast<void *>(scratch), &s);
+    const uint32_t n = num_points;
+    RFB_CUDA(cudaMemcpyAsync(point_adjacency_offsets, s.c, 4 * ((uint64_t)n + 1), cudaMemcpyDeviceToDevice, stream));
+    if (n) {
+        RFB_CUDA(cudaMemsetAsync(s.cursor, 0, 4 * (uint64_t)n, stream));
+        RFB_LAUNCH((delaunay_fill_kernel), blocks_for(n, kDelBlock), kDelBlock, 0, stream, n, order, s.pool, s.start,
+                   s.count, s.c, s.cursor, rows);
+        RFB_LAUNCH((delaunay_sort_kernel), blocks_for(32 * (uint64_t)n, kDelBlock), kDelBlock, 0, stream, n, s.c,
+                   rows, point_adjacency);
+        g_launches += 2;
+    }
+    RFB_CUDA(cudaGetLastError());
     return 0;
 }
 
